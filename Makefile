@@ -1,8 +1,8 @@
-# starway_b200 build (sm_100a only).  `make` builds everything __graft_entry__.build() needs.
+# starway_b200 build (sm_90a only: H100).  `make` builds everything __graft_entry__.build() needs.
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 CC        ?= gcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -cudart static
 CXXFLAGS  := -O2 -g -std=c++17 -fPIC -Wall -Wextra -Wno-unused-parameter -pthread
 CFLAGS    := -O2 -g -std=c11 -fPIC -Wall -Wextra
@@ -52,7 +52,7 @@ build/tagmatch.o: oracle/tagmatch.c oracle/tagmatch.h
 $(ORACLE): build/tagmatch.o
 	$(CC) -shared -o $@ $^
 
-$(CPUENG): oracle/cpu_engine.cpp oracle/tagmatch.c oracle/tagmatch.h
+$(CPUENG): oracle/cpu_engine.cpp build/tagmatch.o oracle/tagmatch.h
 	$(CXX) $(CXXFLAGS) -shared -o $@ oracle/cpu_engine.cpp build/tagmatch.o -lpthread -lrt
 
 build/engine_sim.o: $(ENGINE_SRCS) $(ENGINE_HDRS)

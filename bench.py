@@ -1,11 +1,13 @@
 #!/usr/bin/env python
-"""bench.py — tagged send/recv throughput of starway_b200 (driver contract: see the task brief).
+"""bench.py — tagged send/recv throughput of starway_b200: one JSON result line.
 
-  python bench.py --gpus N --steps K --warmup W            our arm (CUDA, sm_100a)
+  python bench.py --gpus N --steps K --warmup W            our arm (CUDA, sm_90a)
   python bench.py --impl reference --gpus N ...            reference arm: the reference's CPU path
                                                            (restated, oracle/cpu_engine.cpp) on host cores
 Every line also carries `sweep`: BASELINE config 3 sampled at 64 B ... 1 GiB in the same run (--no-sweep skips it;
 the full 25-size sweep, uni- and bidirectional, is `bench_scenarios.py sweep`).
+--dump-outputs DIR writes what the timed path received in its last step (a fixed, seeded sample of every message
+and the (sender_tag, length) results) as .npy files, so that two builds can be compared output for output.
 
 Workload (BASELINE.json configs[1]): point-to-point asend/arecv of 1 MiB buffers, tag=1,
 tag_mask=0xFFFF.  One step = a window of WINDOW messages: the receiver posts WINDOW receives,
@@ -36,10 +38,12 @@ if ROOT not in sys.path:
 
 MSG_BYTES = 1 << 20
 WINDOW = 64
-POOL_SETS = 4  # 4 x 64 MiB sources + 4 x 64 MiB destinations = 512 MiB > 126 MB L2
+POOL_SETS = 4  # 4 x 64 MiB sources + 4 x 64 MiB destinations = 512 MiB > 50 MB L2 (H100)
 TAG, MASK = 1, 0xFFFF
-METRIC = "tagged send/recv GB/s & Mmsg/s vs size, 1/2/4/8 B200; NVLink roofline %"
-NVLINK_NOMINAL_GBS = 900.0  # BASELINE.md: score NVLink against the nominal 900 GB/s per direction (measured peer copy: 770)
+METRIC = "tagged send/recv GB/s & Mmsg/s vs size, 1/2/4/8 H100; NVLink roofline %"
+NVLINK_NOMINAL_GBS = 450.0  # H100 SXM, NVLink 4: 18 links x 25 GB/s per direction (data sheet, not measured)
+HBM_DATASHEET_GBS = 3350.0  # H100 SXM HBM3 data sheet figure; a copy reaches less
+DUMP_ELEMS = 8 << 20  # --dump-outputs: at most this many sampled payload bytes (32 MiB as float32)
 
 
 def new_loop_runner():
@@ -56,7 +60,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
+        return {"hbm_gbs": HBM_DATASHEET_GBS}, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -177,6 +181,21 @@ async def run_sweep(torch, dev, server, client, rank, world, barrier, allreduce_
 
 
 # ----------------------------------------------------------------------------------------- our arm
+def dump_outputs(out_dir, torch, np, dsts, results, suffix):
+    """Writes what the last timed step delivered: `received_sample` (window x k float32, the bytes of every
+    received message at k fixed positions drawn from a seeded generator, k bounded by DUMP_ELEMS), the positions
+    (`sample_index`, float64) and the (sender_tag, length) of every receive (`recv_results`, float64)."""
+    n = dsts[0].numel()
+    k = max(1, min(n, DUMP_ELEMS // len(dsts)))
+    idx = np.sort(np.random.default_rng(0x5EED).choice(n, size=k, replace=False))
+    idx_dev = torch.from_numpy(idx).to(dsts[0].device)
+    sample = torch.stack([d.index_select(0, idx_dev) for d in dsts]).float().cpu().numpy()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"received_sample{suffix}.npy"), sample)
+    np.save(os.path.join(out_dir, f"sample_index{suffix}.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, f"recv_results{suffix}.npy"), np.asarray(results, dtype=np.float64))
+
+
 async def window_step(server, client, eps, srcs, dsts):
     recvs = [server.arecv(d, TAG, MASK) for d in dsts]
     sends = [client.asend(s, TAG) for s in srcs]
@@ -245,11 +264,13 @@ def run_ours(args):
         torch.cuda.synchronize()
 
         async def timed(nsteps, srcs, dsts, sync):
+            res = None
             for i in range(nsteps):
                 k = i % POOL_SETS
                 res = await window_step(server, client, eps, srcs[k], dsts[k])
                 assert all(r == (TAG, msg) for r in res)
             sync()
+            return res
 
         # the set-up garbage (torch import, buffer lists) goes to the permanent generation: full
         # collections inside the timed region would otherwise walk ~10^6 objects (same in the reference arm)
@@ -289,13 +310,16 @@ def run_ours(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         t0 = time.perf_counter()
-        await timed(args.steps, src, dst, torch.cuda.synchronize)
+        last = await timed(args.steps, src, dst, torch.cuda.synchronize)
         t1 = time.perf_counter()
         e1.record()
         e1.synchronize()
         barrier()
         clk = clocks.stop()
         st = ctx.stats()
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, torch, np, dst[(args.steps - 1) % POOL_SETS], last,
+                         "" if world == 1 else f"_rank{rank}")
         dev_ms = e0.elapsed_time(e1)
         wall_ms = (t1 - t0) * 1e3
         ms = max(dev_ms, wall_ms)
@@ -421,19 +445,11 @@ def run_ours(args):
         peak, bound, peak_note = float(peaks["hbm_gbs"]), "hbm", f"HBM copy, {peaks_src}"
     else:
         algo_bytes = payload_per_launch  # N payload bytes cross NVLink in one direction
-        peak, bound, peak_note = NVLINK_NOMINAL_GBS, "nvlink", "NVLink 5 per direction, nominal 900 GB/s (BASELINE.md; measured peer copy on this pool: 770 GB/s)"
+        peak, bound, peak_note = NVLINK_NOMINAL_GBS, "nvlink", f"NVLink 4 per direction, nominal {NVLINK_NOMINAL_GBS:.0f} GB/s (H100 SXM data sheet)"
     achieved = algo_bytes / (avg_ms * 1e-3) / 1e9 if avg_ms > 0 else 0.0
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            tj = json.load(f)
-        if tj.get("world") == world:
-            traffic = tj["dram_bytes_per_payload_byte"] * payload_per_launch
-    except Exception:
-        pass
     roofline = {
         "bound": bound, "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-        "frac": round(achieved / peak, 4), "traffic": traffic,
+        "frac": round(achieved / peak, 4),
         "kernel": kernel,
         "launches": n_launches, "avg_launch_us": round(avg_ms * 1e3, 2),
         "payload_bytes_per_launch": int(payload_per_launch), "peak_source": peak_note,
@@ -477,9 +493,9 @@ def run_ours(args):
         "sweep": {"what": "BASELINE config 3, sampled: per size, `window` messages in flight then aflush, device buffers, "
                           "per direction per GPU" + ("" if world == 1 else f"; every rank streams to rank+1 at once ({world}-GPU ring)"),
                   "roofline_gbs_per_gpu": round(per_gpu_peak, 1),
-                  "roofline": "HBM copy / 2 (loopback: every payload byte is read and written)" if world == 1 else "NVLink 5, 900 GB/s per direction (nominal)",
+                  "roofline": "HBM copy / 2 (loopback: every payload byte is read and written)" if world == 1 else f"NVLink 4, {NVLINK_NOMINAL_GBS:.0f} GB/s per direction (nominal)",
                   "points": sweep},
-        "nvlink_roofline_frac": None if world == 1 else round(value / world / 900.0, 4),
+        "nvlink_roofline_frac": None if world == 1 else round(value / world / NVLINK_NOMINAL_GBS, 4),
         "clocks": clk,
         "e2e": {"value": None if args.no_e2e else round(e2e_value, 2), "unit": "GB/s", "h2d_bytes_per_step": step_bytes, "d2h_bytes_per_step": step_bytes,
                 "buffers": "page-locked host NumPy arrays through Client.asend/Server.arecv", "rank0_breakdown": e2e_diag},
@@ -624,6 +640,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer e2e leg (ncu launch lists of the device-resident steps)")
     ap.add_argument("--no-sweep", action="store_true", help="skip the sampled size sweep (config 3)")
     ap.add_argument("--sweep-max-bytes", type=int, default=1 << 30)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's received data to DIR/*.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

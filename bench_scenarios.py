@@ -8,7 +8,7 @@
 
 Every mode prints one JSON line per data point on rank 0 (and appends it to --out).  Device
 buffers, public asyncio API; GB/s is payload bytes delivered / wall time; `nvlink_frac` is per-GPU
-egress / 900 GB/s (the nominal per-direction NVLink 5 figure named by BASELINE.json).
+egress / 450 GB/s (H100 SXM, NVLink 4: the nominal per-direction figure of the data sheet).
 """
 from __future__ import annotations
 
@@ -19,6 +19,9 @@ import os
 import statistics
 import sys
 import time
+
+NVLINK_NOMINAL_GBS = 450.0  # H100 SXM, NVLink 4, per direction (data sheet)
+HBM_DATASHEET_GBS = 3350.0  # H100 SXM HBM3 (data sheet); a loopback copy moves 2 bytes of HBM per payload byte
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 os.environ.setdefault("STARWAY_QUIET", "1")  # no "Connected!" banners: stdout carries JSON lines only
@@ -167,9 +170,9 @@ def mode_sweep(args):
                         "per_direction": True,
                     }
                     if world > 1:
-                        rec["nvlink_frac_of_900"] = round(rec["gbs_best"] / 900.0, 4)
+                        rec["nvlink_frac"] = round(rec["gbs_best"] / NVLINK_NOMINAL_GBS, 4)
                     else:
-                        rec["hbm_frac"] = round(2 * rec["gbs_best"] / 6575.1, 4)
+                        rec["hbm_frac"] = round(2 * rec["gbs_best"] / HBM_DATASHEET_GBS, 4)
                     if direction == "bi":
                         rec["aggregate_gbs_best"] = round(2 * nbytes / worst / 1e9, 3)
                     emit(args, rec)
@@ -244,7 +247,7 @@ def mode_allpairs(args):
             per_gpu = len(peers) * n * rounds / el / 1e9
             emit(args, {"scenario": "allpairs", "n_gpus": world, "msg_bytes": n, "rounds": rounds,
                         "per_gpu_egress_gbs": round(per_gpu, 2), "aggregate_gbs": round(per_gpu * world, 2),
-                        "nvlink_frac_of_900": round(per_gpu / 900.0, 4), "ms_per_round": round(el / rounds * 1e3, 4)})
+                        "nvlink_frac": round(per_gpu / NVLINK_NOMINAL_GBS, 4), "ms_per_round": round(el / rounds * 1e3, 4)})
         await loop.run_in_executor(None, dist.barrier)
         for c in clients.values():
             await c.aclose()

@@ -1,4 +1,4 @@
-/* starway_b200.h — C ABI of the B200-native tagged-messaging engine.
+/* starway_b200.h — C ABI of the GPU-native (sm_90a) tagged-messaging engine.
  *
  * This is the drop-in boundary for the reference's `_bindings` extension module
  * (reference src/starway/_bindings.pyi:7-88, bound at src/bindings/main.cpp:1538-1581).

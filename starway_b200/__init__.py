@@ -1,8 +1,8 @@
-"""starway_b200 — Blackwell-native tagged point-to-point messaging.
+"""starway_b200 — Hopper-native (H100, sm_90a) tagged point-to-point messaging.
 
 Drop-in for the reference package's public surface (reference
 ``src/starway/__init__.py:351-358``): ``Server``, ``Client``, ``ServerEndpoint``.
-The hot path under it is hand-written sm_100a CUDA reached through the C ABI in
+The hot path under it is hand-written sm_90a CUDA reached through the C ABI in
 ``include/starway_b200.h``; there is NO CPU fallback: if ``libstarway_b200.so``
 is missing this import fails, and if no CUDA device is visible the first
 ``Server()`` / ``Client()`` raises.

@@ -264,7 +264,7 @@ struct StagingPool {
 
 // ============================================================================ pageable host buffers
 // cudaMemcpyAsync from / to pageable memory is a synchronous, single-threaded staging loop inside the driver
-// (~6 GB/s on the B200 hosts, and it blocks the progress thread).  Large pageable buffers are moved by a few
+// (slow, and it blocks the progress thread).  Large pageable buffers are moved by a few
 // helper threads between the caller's memory and page-locked staging instead (chunked memcpy), and the copy
 // engine only ever sees page-locked memory.  The payload still travels host -> GPU -> (NVLink) -> GPU -> host.
 struct CopyPool {
@@ -778,7 +778,7 @@ struct Ctx {
   // byte range (sw_bulk_tma_jobs_kernel); 0: segment list in pinned host memory (sw_bulk_tma_kernel)
   std::atomic<int64_t> opt_bulk_balance{1};
   // small put / match launches announce completion through a flag in pinned host memory
-  // (launch -> seen 7.4 us vs 15.2 us through a timing event on B200, profiles/r01_probe_floor.log)
+  // (seen sooner than through a timing event; `sw_probe floor` measures both)
   std::atomic<int64_t> opt_done_flags{1};
   uint64_t flag_seq = 0;
   std::atomic<int64_t> opt_heap_small{4096}, opt_heap_big{512};
@@ -788,8 +788,7 @@ struct Ctx {
   std::atomic<int64_t> opt_pinned_send_direct{1};
   std::atomic<int64_t> opt_pull_keep_us{60};   // the pull kernel stays through gaps between needs up to this long (0: asked to leave at once)
   // 1: upload pinned host sources with the TMA bulk kernel; 0 (default): copy engine (cudaMemcpyAsync).
-  // Measured on B200 (profiles/r01_e2e_staging_variants.md): the copy engine leaves the SMs and more of
-  // the PCIe duplex budget to the concurrent download kernel (43.8 vs 37.9 GB/s at N=2).
+  // The copy engine leaves the SMs and more of the PCIe duplex budget to the concurrent download kernel.
   std::atomic<int64_t> opt_stage_upload_kernel{0};
   std::atomic<int64_t> opt_stage_batch_bytes{(int64_t)STAGE_BATCH_BYTES};   // staged sends are announced in batches of this size
   std::atomic<int64_t> opt_max_mappings{(int64_t)MAX_MAPPINGS};   // peer allocations kept mapped (LRU quarter dropped when full)
@@ -2885,7 +2884,7 @@ void check_flushes(Ctx* c, Worker* w) {
 
 void worker_release(Ctx* c, Worker* w, bool leak_rings) {
   if (c->tracing && w->pctl && w->pctl->dbg[0]) {
-    const double mhz = 1965.0, n = (double)w->pctl->dbg[0];
+    const double mhz = (double)swgpu::clock_mhz(), n = (double)w->pctl->dbg[0];
     fprintf(stderr, "starway_b200 resident puts (worker %llx): %llu; seen->staged %.2f us, staged->released %.2f us, released->published %.2f us; link round %.2f us\n",
             (unsigned long long)w->id, (unsigned long long)w->pctl->dbg[0], w->pctl->dbg[1] / n / mhz, w->pctl->dbg[2] / n / mhz,
             w->pctl->dbg[3] / n / mhz, w->pctl->dbg[4] ? w->pctl->dbg[5] / (double)w->pctl->dbg[4] / mhz : 0.0);
@@ -3133,8 +3132,8 @@ void drain_sq(Ctx* c) {
 // ============================================================================ NUMA placement
 // GPU-local CPUs from sysfs (what `nvidia-smi topo -m` prints as CPU affinity).  Pinned control
 // blocks and staging buffers are allocated, and the progress thread runs, next to the GPU's PCIe
-// root: on the 2-socket B200 boxes a rank whose host memory sits on the other socket moves its
-// host<->device traffic over UPI (measured: per-GPU e2e rate halves from N=2 to N=4).
+// root: on a 2-socket host a rank whose host memory sits on the other socket moves its
+// host<->device traffic over the inter-socket link.
 std::string device_cpulist(int device) {
   char bus[64];
   if (swgpu::device_pci_bus_id(device, bus, sizeof bus) != 0) return "";
@@ -3956,8 +3955,8 @@ int sw_ep_info_get(sw_ctx* ctx, sw_worker_t wid, sw_ep_t epid, sw_ep_info* out) 
 }
 
 // reference evaluate_perf (main.cpp:452-467, 666-678) returns UCX's analytic time estimate for a
-// message size.  Here: latency + size / bandwidth with constants fitted to the measured curves
-// (profiles/r01_pingpong_*.jsonl one-way latencies, r01_sweep_*.jsonl asymptotic bandwidths), seconds.
+// message size.  Here: latency + size / bandwidth, with the latencies of `bench_scenarios.py pingpong` and the
+// 1 GiB loopback rate of the bench sweep, measured on one H100 SXM (80 GB, 400 W power limit), seconds.
 double sw_evaluate_perf(sw_ctx* ctx, sw_worker_t wid, sw_ep_t epid, size_t msg_size) {
   Ctx* c = (Ctx*)ctx;
   Worker* w = find_worker(c, wid);
@@ -3968,14 +3967,13 @@ double sw_evaluate_perf(sw_ctx* ctx, sw_worker_t wid, sw_ep_t epid, size_t msg_s
   Ep* ep = epid ? find_ep(c, epid) : (w->eps.empty() ? nullptr : w->eps[0]);
   const bool same_gpu = !ep || ep->in_process || ep->peer_device == c->device;
   const bool eager = msg_size <= (size_t)c->opt_eager_max.load();
-  // Measured on B200 through the asyncio API (profiles/r02_pingpong_*): one-way 64 B 12.7 us on one GPU, 13.3 us over
-  // NVLink; a rendezvous adds the pull hand-over and the completion records (1 MiB: 25.8 / 26.7 us one-way).  With the
-  // discrete-kernel engine (resident=0) the round-1 figures apply.
+  // One-way latency through the asyncio API on one GPU: 64 B 29.9 us, 1 MiB 52.3 us (resident=0: 64.3 / 91.5 us).
+  // A peer over NVLink has not been measured on H100; its estimate takes the same latency.
   const bool resident = c->opt_resident.load() != 0;
-  const double lat = resident ? (same_gpu ? (eager ? 12.7e-6 : 25.5e-6) : (eager ? 13.3e-6 : 25.3e-6))
-                              : (same_gpu ? (eager ? 47e-6 : 62e-6) : (eager ? 49e-6 : 68e-6));
-  // copy rate of one large message: HBM copy on one GPU (3.3 TB/s payload), NVLink pull between GPUs (0.65 TB/s)
-  const double bw = same_gpu ? 3.3e12 : 6.5e11;
+  const double lat = resident ? (eager ? 29.9e-6 : 52.3e-6) : (eager ? 64.3e-6 : 91.5e-6);
+  // copy rate of one large message: HBM copy on one GPU (1.16 TB/s payload at 1 GiB, measured), NVLink 4 pull
+  // between GPUs (450 GB/s per direction, nominal: not measured)
+  const double bw = same_gpu ? 1.16e12 : 4.5e11;
   return lat + (double)msg_size / bw;
 }
 

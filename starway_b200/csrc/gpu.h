@@ -1,6 +1,6 @@
 // starway_b200 — the narrow interface between the host progress engine
 // (engine.cpp) and the device backend.  The product backend is gpu_cuda.cu
-// (hand-written sm_100a kernels).  tests/hostsim/gpu_sim.cpp is a test-only
+// (hand-written sm_90a kernels).  tests/hostsim/gpu_sim.cpp is a test-only
 // stand-in that lets the CPU test-suite exercise the host protocol logic
 // without a GPU; it is never linked into the product library.
 #pragma once
@@ -37,6 +37,7 @@ int device_count();
 int init(int device);                 // binds the calling thread to `device`
 int bind_thread(int device);          // cudaSetDevice for helper threads
 int sm_count();
+int clock_mhz();                       // SM clock that converts device cycle counts to time
 int device_pci_bus_id(int device, char* out, int cap);   // "0000:1b:00.0"; < 0 when unknown
 
 void* dev_alloc(size_t bytes);        // IPC-shareable device allocation, zeroed
@@ -62,8 +63,8 @@ int event_sync(event_t e);
 float event_elapsed_ms(event_t a, event_t b);
 
 int memcpy_h2d(void* dst, const void* src, size_t n, stream_t s);
-// n host -> device copies as ONE copy-engine submission (cudaMemcpyBatchAsync): separate 1 MiB copies reach 28 GB/s while
-// the other direction of the link is busy, the batch 49 GB/s (profiles/r02_probe_duplex_patterns.txt)
+// n host -> device copies as ONE copy-engine submission (cudaMemcpyBatchAsync): separate 1 MiB copies each pay a start-up
+// cost that grows while the other direction of the link is busy, the batch pays it once (`sw_probe duplex` compares them)
 int memcpy_h2d_batch(void* const* dsts, const void* const* srcs, const size_t* sizes, size_t n, stream_t s);
 int memcpy_batch(void* const* dsts, const void* const* srcs, const size_t* sizes, size_t n, stream_t s);   // any direction
 int memcpy_d2h(void* dst, const void* src, size_t n, stream_t s);

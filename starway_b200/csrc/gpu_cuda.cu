@@ -1,5 +1,5 @@
-// starway_b200 — CUDA (sm_100a) implementation of the swgpu backend interface.
-// Compiled with: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo
+// starway_b200 — CUDA (sm_90a) implementation of the swgpu backend interface.
+// Compiled with: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <string.h>
@@ -16,9 +16,10 @@
 namespace swgpu {
 
 static thread_local std::string g_err;
-static int g_sms = 148;
+static int g_sms = 132;
 static int g_max_smem_optin = 0;
-static int g_clk_mhz = 1965;
+static int g_smem_per_sm = 228 * 1024;
+static int g_clk_mhz = 1980;
 
 static int fail(cudaError_t e, const char* what) {
   char buf[256];
@@ -33,7 +34,7 @@ static int fail(cudaError_t e, const char* what) {
     if (e__ != cudaSuccess) return fail(e__, #call); \
   } while (0)
 
-const char* backend_name() { return "cuda-sm_100a"; }
+const char* backend_name() { return "cuda-sm_90a"; }
 const char* last_error() { return g_err.c_str(); }
 
 int device_count() {
@@ -61,6 +62,7 @@ int init(int device) {
   SW_CUDA(cudaGetDeviceProperties(&prop, device));
   g_sms = prop.multiProcessorCount;
   g_max_smem_optin = (int)prop.sharedMemPerBlockOptin;
+  g_smem_per_sm = (int)prop.sharedMemPerMultiprocessor;
   {
     int khz = 0;
     if (cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, device) == cudaSuccess && khz > 0) g_clk_mhz = khz / 1000;
@@ -83,6 +85,7 @@ int bind_thread(int device) {
   return 0;
 }
 int sm_count() { return g_sms; }
+int clock_mhz() { return g_clk_mhz; }
 int device_pci_bus_id(int device, char* out, int cap) {
   if (cap < 16) return -1;
   cudaError_t r = cudaDeviceGetPCIBusId(out, cap, device);
@@ -486,7 +489,7 @@ int launch_bulk(stream_t s, const SwSeg* segs, uint32_t nseg, const BulkTuning* 
       return -1;
     }
     int ctas = t->ctas_per_sm > 0 ? t->ctas_per_sm : 1;
-    const int fit = (int)((size_t)(228 * 1024) / (smem + 1024 + 128));   // CTAs of this size resident per SM
+    const int fit = (int)((size_t)g_smem_per_sm / (smem + 1024 + 128));   // CTAs of this size resident per SM
     if (ctas > fit) ctas = fit < 1 ? 1 : fit;
     uint32_t grid = (uint32_t)(g_sms * ctas);
     SwBulkJobArgs ja;

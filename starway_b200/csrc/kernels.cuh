@@ -1,4 +1,4 @@
-// starway_b200 — hand-written sm_100a kernels for the tagged-messaging hot path.
+// starway_b200 — hand-written sm_90a kernels for the tagged-messaging hot path.
 //
 //   sw_put_kernel       eager / RTS put: vectorised stores into the peer's inbound ring
 //   sw_put_inline_kernel  same, descriptors + RTS payloads as kernel parameters (batches <= 32)
@@ -188,8 +188,7 @@ struct SwPutArgs {
 static_assert(sizeof(SwPutArgs) <= 4096, "inline put parameters");
 // ONE CTA, one warp per message.  Completion is announced by a flag in pinned host memory: the
 // barrier collects every warp's stores, thread 0's system-scope fence orders them (cumulatively)
-// before the flag.  Measured on B200 (`sw_probe floor`): launch -> flag seen 7.4 us, launch -> timing
-// event seen 15.2 us.
+// before the flag, which the host sees sooner than a timing event (`sw_probe floor` measures both).
 __global__ void __launch_bounds__(SW_PUT_INLINE * 32) sw_put_inline_kernel(const __grid_constant__ SwPutArgs a) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp = threadIdx.x >> 5;
@@ -975,8 +974,8 @@ __global__ void __launch_bounds__(32) sw_bulk_tma_kernel(const SwSeg* __restrict
 // Launches with few segments carry the list in the kernel parameter bank: the first bulk load of
 // every CTA is not preceded by a read of pinned host memory over PCIe.
 // Only the latency-critical small launches take this route: the parameter block stays under the
-// classic 4 KiB limit.  Measured on B200: a 24 KiB parameter block (768 segments) made every
-// launch cost more on the host than the first-segment PCIe read it saved (bench N=2 360 -> 227 GB/s).
+// classic 4 KiB limit: a much larger parameter block costs more host time per launch than the
+// first-segment PCIe read it saves.
 constexpr uint32_t SW_BULK_INLINE_SEGS_SMALL = 96;   // 3 KiB
 template <uint32_t N>
 struct SwSegArgs {

@@ -1,4 +1,4 @@
-// starway_b200 — resident progress kernels (sm_100a): the receive side without the host on the data path.
+// starway_b200 — resident progress kernels (sm_90a): the receive side without the host on the data path.
 //
 //   sw_progress_kernel  ONE CTA per worker (Client / Server object), resident for a bounded time:
 //                         warp 0   matcher: polls the slot headers of the inbound rings (ld.acquire.sys on the

@@ -1,4 +1,4 @@
-// starway_b200 — layouts shared by the host progress engine and the sm_100a kernels.
+// starway_b200 — layouts shared by the host progress engine and the sm_90a kernels.
 //
 // Everything in this file is plain-old-data that lives either in device memory
 // (rings, queues, job lists), in pinned host memory (per-launch input/output

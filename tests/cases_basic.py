@@ -2,7 +2,7 @@
 
 Every coroutine below takes ``api`` — a namespace with ``Server`` / ``Client`` — so the
 same case runs (a) against the host-logic simulator on CPU and (b) against the CUDA
-library on the B200.  Each case cites the reference test it restates.  The reference
+library on the GPU.  Each case cites the reference test it restates.  The reference
 uses pytest-asyncio (absent here): the runners wrap the coroutines in ``asyncio.run``.
 
 Not portable, and why:

@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with `-m gpu`)")
     # the native pieces are built in-tree by `make` (== __graft_entry__.build()); build them on demand
     needed = ["starway_b200/libstarway_b200.so", "starway_b200/_fastpath.so", "oracle/liboracle_tagmatch.so",
               "oracle/libstarway_cpu.so", "tests/hostsim/libstarway_hostsim.so"]
@@ -53,7 +53,7 @@ def sim_api():
 
 @pytest.fixture(scope="session")
 def cuda_api():
-    """API classes bound to the product library (CUDA, sm_100a)."""
+    """API classes bound to the product library (CUDA, sm_90a)."""
     import types
 
     import starway_b200 as sw

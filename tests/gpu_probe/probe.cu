@@ -1,5 +1,5 @@
 // tests/gpu_probe/probe.cu — GPU-side unit tests and micro-benchmarks for the starway_b200
-// kernels (TEST INFRASTRUCTURE).  Runs on a B200 box via gpurun:
+// kernels (TEST INFRASTRUCTURE).  Needs a GPU (built for sm_90a by `make probe`):
 //   sw_probe correctness           bulk-copy + put/match/deliver parity vs oracle/tagmatch.c
 //   sw_probe bench                 single-GPU bulk copy bandwidth sweep (TMA vs SIMT tunings)
 //   sw_probe peer                  2-GPU in-process peer pull/push bandwidth, cudaMemcpyPeer ceiling
@@ -1256,7 +1256,7 @@ static void bench_pull(FILE* json, int nbatches_fixed) {
     const uint32_t nb = nbatches_fixed ? (uint32_t)nbatches_fixed : sh.nbatch;
     uint64_t s0[8], s1[8];
     pull_queue_read_stats(q, s0);
-    // (L2 is 126 MB: batches of a shape use disjoint parts of the 2 GiB pools, wrapping)
+    // (larger than the 50 MB L2 of an H100: batches of a shape use disjoint parts of the 2 GiB pools, wrapping)
     uint64_t off = 0;
     for (uint32_t b = 0; b < nb; b++) {
       SwSeg* m = msgs + (size_t)b * SW_PULL_JOBS;

@@ -67,6 +67,7 @@ int init(int device) {
 }
 int bind_thread(int) { return 0; }
 int sm_count() { return 8; }
+int clock_mhz() { return 1000; }
 int device_pci_bus_id(int, char*, int) { return -1; }
 
 static void cleanup_all() {
@@ -480,7 +481,7 @@ int launch_bulk(stream_t, const SwSeg* segs, uint32_t nseg, const BulkTuning* t)
   SwBulkJobArgs ja;
   uint32_t grid = 0;
   if (t && t->mode == 0 && t->balance &&
-      bulk_build_jobs(segs, nseg, 148, (uint32_t)(t->stage_bytes & ~15), (uint32_t)t->stages, &ja, &grid)) {
+      bulk_build_jobs(segs, nseg, 132, (uint32_t)(t->stage_bytes & ~15), (uint32_t)t->stages, &ja, &grid)) {
     if (getenv("SW_SIM_TRACE_BULK")) fprintf(stderr, "simjobs njobs=%u grid=%u share=%llu total=%llu\n", ja.njobs, grid, (unsigned long long)ja.share, (unsigned long long)ja.end[ja.njobs - 1]);
     uint64_t copied = 0, want = ja.end[ja.njobs - 1];
     for (uint32_t cta = 0; cta < grid; cta++) {

@@ -28,7 +28,7 @@ def test_product_library_exports_the_abi():
     for name in header_symbols():
         assert hasattr(lib, name), name
     assert sw._api.lib.sw_abi_version() == 1
-    assert sw.backend_name() == "cuda-sm_100a"
+    assert sw.backend_name() == "cuda-sm_90a"
     assert sw.status_string(-16) == "Request canceled"
     assert sw.status_string(-24) == "Endpoint is not connected"
     assert sw.status_string(-9) == "Message truncated"

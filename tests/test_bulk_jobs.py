@@ -1,5 +1,5 @@
 """Host-side check of the balanced bulk launch: `bulk_build_jobs` (starway_b200/csrc/bulk_jobs.h) and the
-per-CTA byte-range iterator `SwJobRangeIter` (sw_device.h) that the sm_100a kernel
+per-CTA byte-range iterator `SwJobRangeIter` (sw_device.h) that the sm_90a kernel
 `sw_bulk_tma_jobs_kernel` runs unchanged.  A C++ harness (compiled here with g++) replays every CTA of
 randomized launches on the CPU and checks: every byte copied exactly once, pieces 16-byte aligned,
 within one job, at most stage_bytes long, grid <= max CTAs, shares equal within 1 KiB."""

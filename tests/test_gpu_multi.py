@@ -1,8 +1,8 @@
 """Multi-GPU parity (one process per GPU, NVLink peer path): BASELINE configs 2-5 at test size, every
 received byte and every (sender_tag, length) checked against the CPU oracle (tests/multi_gpu_worker.py).
 
-Skipped when the box has fewer GPUs than the test's world size: `gpurun --gpus 2` runs the world-2 case,
-`gpurun --gpus 8` runs worlds 2, 4 and 8.  Logs of those runs are committed under profiles/."""
+Skipped when the machine has fewer GPUs than the test's world size: a 2-GPU machine runs the world-2 case,
+an 8-GPU machine worlds 2, 4 and 8."""
 import multiprocessing as mp
 import queue as queue_mod
 

@@ -1,5 +1,5 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).  Everything here goes through
-the C ABI of libstarway_b200.so (ctypes) into the sm_100a kernels; results are compared
+"""GPU parity tests (run on a GPU machine: `pytest -m gpu`).  Everything here goes through
+the C ABI of libstarway_b200.so (ctypes) into the sm_90a kernels; results are compared
 bit-exactly with the CPU oracle (oracle/tagmatch.*), with the golden vectors transcribed
 from the reference's tests, and through size-independent properties at full sizes."""
 import asyncio
@@ -30,7 +30,7 @@ def torch_cuda():
 
 def test_product_library_is_cuda(cuda_api):
     # the product path must be the CUDA extension, never a CPU stand-in
-    assert cuda_api.backend_name() == "cuda-sm_100a"
+    assert cuda_api.backend_name() == "cuda-sm_90a"
     torch_cuda()
 
 
@@ -506,7 +506,7 @@ def test_completion_detection_modes(cuda_api, port, opts):
 
 def test_pingpong_latency_small_messages(cuda_api, port):
     """Latency regression guard for the flag-based completion path: a 64 B device-buffer round trip
-    through the public API stays well under 200 us (measured ~50 us on B200)."""
+    through the public API stays well under 400 us (median ~60 us on an H100 SXM at 400 W)."""
     import time
 
     torch = torch_cuda()
@@ -526,7 +526,7 @@ def test_pingpong_latency_small_messages(cuda_api, port):
                 await server.asend(ep, pong, 2)
                 await f
                 samples.append(time.perf_counter() - t0)
-            # best block median: robust against a busy host; measured ~50 us on B200, bound is generous
+            # best block median: robust against a busy host; ~60 us on an H100 SXM, bound is generous
             med = min(sorted(samples[k:k + 50])[25] for k in range(50, 300, 50))
             print(f"64 B device ping-pong RTT median {med * 1e6:.1f} us")
             assert med < 400e-6
@@ -574,7 +574,7 @@ def test_bench_cli_loopback_all_scenarios(tmp_path, buffers):
     assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-2000:]
     report = json.loads(out.read_text())
     check_report(report, with_samples=True)
-    assert report["transport"] == f"cuda-sm_100a:{buffers}"
+    assert report["transport"] == f"cuda-sm_90a:{buffers}"
     m = {s["name"]: s["metrics"] for s in report["scenarios"]}
     assert m["large-array"]["avg_gbps"] > 1.0 and m["small-messages"]["messages_per_second"] > 1e4
     assert 0 < m["pingpong-flag"]["median_rtt_us"] < 5000 and m["streaming-duplex"]["aggregate_gbps"] > 1.0

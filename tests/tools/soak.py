@@ -1,6 +1,6 @@
 """Leak / stability soak: repeated listen / connect / mixed traffic / close cycles.
   python tests/tools/soak.py sim 200      CPU host-logic simulator
-  python tests/tools/soak.py cuda 200     B200 (prints device memory in use)
+  python tests/tools/soak.py cuda 200     CUDA device (prints device memory in use)
 Reports file descriptors, POSIX-shm segments, resident set and (cuda) device memory per 50 cycles;
 all of them must stay flat."""
 import asyncio
