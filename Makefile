@@ -69,8 +69,8 @@ build/gpu_sim.o: tests/hostsim/gpu_sim.cpp $(CSRC)/gpu.h $(CSRC)/sw_device.h $(C
 $(HOSTSIM): build/engine_sim.o build/gpu_sim.o build/tagmatch.o
 	$(CXX) -shared -Wl,-Bsymbolic -Wl,--version-script=tests/hostsim/exports_sim.map -o $@ $^ -lpthread -lrt -ldl
 
-$(PROBE): tests/gpu_probe/probe.cu build/gpu_cuda.o build/tagmatch.o
-	$(NVCC) $(NVFLAGS) -o $@ tests/gpu_probe/probe.cu build/gpu_cuda.o build/tagmatch.o
+$(PROBE): tests/gpu_probe/probe.cu build/gpu_cuda.o
+	$(NVCC) $(NVFLAGS) -o $@ tests/gpu_probe/probe.cu build/gpu_cuda.o
 
 $(ABIBENCH): tests/gpu_probe/abi_bench.cpp $(LIB) include/starway_b200.h
 	$(CXX) -O2 -std=c++17 -I/usr/local/cuda/include -o $@ tests/gpu_probe/abi_bench.cpp -Lstarway_b200 -lstarway_b200 -L/usr/local/cuda/lib64 -lcudart -Wl,-rpath,'$$ORIGIN/../../starway_b200' -Wl,-rpath,/usr/local/cuda/lib64

@@ -317,8 +317,7 @@ def mode_storm(args):
                         "kernel_level": {
                             "put_msgs": st["put_msgs"], "put_launches": st["put_launches"],
                             "put_mmsg_s": round(st["put_msgs"] / max(st["put_event_ms"], 1e-9) / 1e3, 2),
-                            "match_arrivals": st["match_arrivals"], "match_launches": st["match_launches"],
-                            "match_mmsg_s": round(st["match_arrivals"] / max(st["match_event_ms"], 1e-9) / 1e3, 2),
+                            "match_arrivals": st["match_arrivals"],
                             "note": "rank 0 counters; device time of the launches from CUDA events"}})
         await loop.run_in_executor(None, dist.barrier)
         for c in clients.values():

@@ -87,7 +87,8 @@ typedef struct sw_ep_info {
 
 typedef struct sw_stats {
   uint64_t put_launches, put_msgs, put_bytes;
-  uint64_t match_launches, deliver_launches, match_posts, match_arrivals;
+  uint64_t match_launches, deliver_launches;   /* always 0: receives are matched by the resident control kernels */
+  uint64_t match_posts, match_arrivals;       /* receives handed to the device, ring slots consumed */
   uint64_t bulk_tma_launches, bulk_simt_launches, bulk_jobs, bulk_bytes;
   uint64_t h2d_bytes, d2h_bytes;
   uint64_t completions;
@@ -96,7 +97,7 @@ typedef struct sw_stats {
   uint64_t bulk_event_bytes;
   double put_event_ms;
   uint64_t put_event_launches;
-  double match_event_ms;      /* match + deliver pair */
+  double match_event_ms;      /* always 0, like match_launches */
   uint64_t match_event_launches;
   /* resident path: control-kernel / pull-kernel launches, and what the pull CTAs copied (bytes) in how much
    * time (union of the batches' active intervals, device timer) -- the roofline numerator / denominator */

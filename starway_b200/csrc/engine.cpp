@@ -6,10 +6,11 @@
 //   * drains a submission queue filled by sw_post_* (reference Channel<T> mailboxes, chan.hpp:84-120),
 //   * batches sends into sw_put_kernel launches (eager payloads / RTS descriptors stored straight
 //     into the peer's device-resident inbound ring through a CUDA-IPC mapping),
-//   * feeds new receives and ring arrivals to sw_match_kernel + sw_deliver_kernel
-//     (device-resident posted/unexpected queues),
-//   * turns rendezvous matches into sw_bulk_*_kernel launches that PULL the payload from the
-//     sender's buffer (IPC mapping) into the caller's receive buffer,
+//   * feeds new receives to the resident control kernel of each worker (sw_progress_kernel), which
+//     matches them against ring arrivals in device-resident posted/unexpected queues,
+//   * keeps the resident pull CTAs (sw_pull_kernel) alive while rendezvous payloads are to be PULLED from
+//     the sender's buffer (IPC mapping) into the caller's receive buffer, and turns the rendezvous matches
+//     the device leaves to the host into sw_bulk_*_kernel launches,
 //   * resolves operations by polling CUDA events (replaces ucp_worker_progress + UCX callbacks).
 // Host<->host signalling (doorbells, credits, FIN/CLOSE) uses a small POSIX shared-memory
 // control block per connection; the worker-address handshake (main.cpp:292-317, 912-985)
@@ -573,21 +574,10 @@ struct Worker {
   std::atomic<int> status{SW_ST_VOID};
   // device-resident queues
   SwMatchState* mstate = nullptr;
-  SwMatchIn* min = nullptr;
-  SwMatchOut* mout = nullptr;
-  swgpu::event_t mev = nullptr, mev_start = nullptr, mev_fast = nullptr;
-  uint64_t mdone_seq = 0;
-  uint32_t mspins = 0;
-  bool mflag_mode = false, mtimed = false;
-  bool match_inflight = false;
-  uint32_t match_posts_inflight = 0;
-  uint64_t stall_unseen = 0;
-  SwMatchScalars msc;       // queue cursors reported by the last match launch (handed back by value)
   std::vector<Ep*> eps;  // index == Ep::index
   // receives
   std::deque<RecvOp*> new_posts;
   std::unordered_map<uint64_t, RecvOp*> recvs;  // handed to the device, not completed
-  uint32_t posted_est = 0;
   // flush
   std::vector<FlushOp*> flushes;
   // listeners
@@ -611,7 +601,6 @@ struct Worker {
   std::thread connector;
   uint32_t bulk_inflight = 0;
   // ---- resident path (sw_progress_kernel): host-visible rings and control words of this worker
-  bool resident = false;
   SwProgCtl* pctl = nullptr;
   SwPostEnt* post_ring = nullptr;
   SwCqEnt* cq_ring = nullptr;
@@ -749,7 +738,7 @@ struct Ctx {
   std::vector<Worker*> active;  // progress-thread private
   bool need_prune = false;      // progress-thread private: a worker reached close phase 4
   // device resources
-  swgpu::stream_t s_put = nullptr, s_match = nullptr, s_bulk = nullptr;
+  swgpu::stream_t s_put = nullptr, s_bulk = nullptr;
   PutBlock put_blocks[N_PUT_BLOCKS];
   uint32_t put_head = 0, put_tail = 0;  // ring of in-flight put blocks
   BulkBlock bulk_blocks[N_BULK_BLOCKS];
@@ -777,7 +766,7 @@ struct Ctx {
   // 1: launches of <= 96 messages carry the messages as kernel parameters and every CTA copies an equal
   // byte range (sw_bulk_tma_jobs_kernel); 0: segment list in pinned host memory (sw_bulk_tma_kernel)
   std::atomic<int64_t> opt_bulk_balance{1};
-  // small put / match launches announce completion through a flag in pinned host memory
+  // small put launches announce completion through a flag in pinned host memory
   // (seen sooner than through a timing event; `sw_probe floor` measures both)
   std::atomic<int64_t> opt_done_flags{1};
   uint64_t flag_seq = 0;
@@ -794,10 +783,8 @@ struct Ctx {
   std::atomic<int64_t> opt_max_mappings{(int64_t)MAX_MAPPINGS};   // peer allocations kept mapped (LRU quarter dropped when full)
   std::atomic<int64_t> opt_hostdst_ce{0};    // device -> pinned-host copies by the copy engine (batched) instead of a kernel
   std::atomic<int64_t> opt_hostdst_tma{0};   // device -> pinned-host copies by the TMA kernel instead of the SIMT kernel
-  // ---- resident path
-  // 1: receives are driven by resident control kernels (sw_progress_kernel) and rendezvous copies by the
-  // resident pull CTAs (sw_pull_kernel); 0: one match launch per batch, host-launched bulk copies (round 1)
-  std::atomic<int64_t> opt_resident{1};
+  // ---- resident path: receives are driven by resident control kernels (sw_progress_kernel) and rendezvous
+  // copies by the resident pull CTAs (sw_pull_kernel)
   std::atomic<int64_t> opt_linger_us{150}, opt_max_life_us{2000}, opt_armed_ms{30}, opt_pull_ctas{0};
   // batches of at most this many sends of ONE worker whose control kernel is resident are executed by that
   // kernel (descriptor ring in pinned memory) instead of a put launch; 0: always launch
@@ -975,43 +962,26 @@ bool worker_alloc_device(Ctx* c, Worker* w) {
     set_error(std::string("match_state_create: ") + swgpu::last_error());
     return false;
   }
-  w->min = (SwMatchIn*)swgpu::host_alloc(sizeof(SwMatchIn));
-  w->mout = (SwMatchOut*)swgpu::host_alloc(sizeof(SwMatchOut));
-  w->mev = swgpu::event_create(1);
-  w->mev_start = swgpu::event_create(1);
-  w->mev_fast = swgpu::event_create(0);
-  memset(&w->msc, 0, sizeof(w->msc));
-  w->msc.n_free_small = (uint32_t)c->opt_heap_small.load();
-  w->msc.n_free_big = (uint32_t)c->opt_heap_big.load();
-  w->msc.valid = 1;
-  if (!w->min || !w->mout || !w->mev) {
-    set_error(std::string("worker pinned alloc: ") + swgpu::last_error());
+  w->pctl = (SwProgCtl*)swgpu::host_alloc(sizeof(SwProgCtl));
+  w->post_ring = (SwPostEnt*)swgpu::host_alloc(sizeof(SwPostEnt) * SW_POST_RING);
+  w->cq_ring = (SwCqEnt*)swgpu::host_alloc(sizeof(SwCqEnt) * SW_CQ_RING);
+  w->cqr_ring = (SwCqEnt*)swgpu::host_alloc(sizeof(SwCqEnt) * SW_CQ_RING);
+  w->hr_ring = (SwHrEnt*)swgpu::host_alloc(sizeof(SwHrEnt) * SW_HR_RING);
+  w->send_ring = (SwSendLL*)swgpu::host_alloc(sizeof(SwSendLL) * SW_SEND_RING);
+  if (w->send_ring) memset(w->send_ring, 0, sizeof(SwSendLL) * SW_SEND_RING);   // stamp 0: never an entry
+  w->s_ctl = swgpu::stream_create();
+  if (!w->pctl || !w->post_ring || !w->cq_ring || !w->cqr_ring || !w->hr_ring || !w->send_ring || !w->s_ctl) {
+    set_error(std::string("worker resident-path alloc: ") + swgpu::last_error());
     return false;
   }
-  w->resident = c->opt_resident.load() != 0 && c->pq && c->map_tbl;
-  if (w->resident) {
-    w->pctl = (SwProgCtl*)swgpu::host_alloc(sizeof(SwProgCtl));
-    w->post_ring = (SwPostEnt*)swgpu::host_alloc(sizeof(SwPostEnt) * SW_POST_RING);
-    w->cq_ring = (SwCqEnt*)swgpu::host_alloc(sizeof(SwCqEnt) * SW_CQ_RING);
-    w->cqr_ring = (SwCqEnt*)swgpu::host_alloc(sizeof(SwCqEnt) * SW_CQ_RING);
-    w->hr_ring = (SwHrEnt*)swgpu::host_alloc(sizeof(SwHrEnt) * SW_HR_RING);
-    w->send_ring = (SwSendLL*)swgpu::host_alloc(sizeof(SwSendLL) * SW_SEND_RING);
-    if (w->send_ring) memset(w->send_ring, 0, sizeof(SwSendLL) * SW_SEND_RING);   // stamp 0: never an entry
-    w->s_ctl = swgpu::stream_create();
-    if (!w->pctl || !w->post_ring || !w->cq_ring || !w->cqr_ring || !w->hr_ring || !w->send_ring || !w->s_ctl) {
-      set_error(std::string("worker resident-path alloc: ") + swgpu::last_error());
-      return false;
-    }
-    w->last_activity = now_s();
-  }
+  w->last_activity = now_s();
   return true;
 }
 
 // per-endpoint words the control kernel publishes to: the sender-visible credit word and the FIN words of the
 // inbound direction, through the page-locked alias of the control block
 bool ep_publish_words(Worker* w, Ep* ep) {
-  if (!w->resident) return true;
-  if (!ep->shm_dev) return false;   // sw_ctx_create probed page-locking: this is an error, not a mode switch
+  if (!ep->shm_dev) return false;   // sw_ctx_create probed page-locking: this is an error
   const size_t off = (uint8_t*)ep->in - (uint8_t*)ep->shm;
   return swgpu::match_state_set_ep_words(w->mstate, ep->index, ep->shm_dev + off + offsetof(ShmDir, consumed),
                                          ep->shm_dev + off + offsetof(ShmDir, gfin)) == 0;
@@ -1069,7 +1039,7 @@ ShmCtl* shm_adopt(const std::string& name, void* p, size_t sz, uint8_t** dev_out
   m.size = sz;
   m.refs = 1;
   m.dev = (uint8_t*)swgpu::host_register(p, sz);
-  if (!m.dev) fprintf(stderr, "starway_b200: control block not page-locked (%s): receives fall back to host-driven launches\n", swgpu::last_error());
+  if (!m.dev) fprintf(stderr, "starway_b200: control block not page-locked (%s)\n", swgpu::last_error());
   g_shm[name] = m;
   *dev_out = m.dev;
   return m.host;
@@ -1782,7 +1752,7 @@ bool pump_sends(Ctx* c) {
   // ---- small batch of one worker whose control kernel is resident: hand the descriptors to that kernel
   if (n <= (uint32_t)c->opt_resident_puts.load() && !stream_ordered && b.nsegs == 0 && swgpu::resident_lingers()) {
     Worker* w0 = b.items[0].op->w;
-    bool one = w0->resident && w0->prog_running && w0->send_ring && c->opt_profile.load() < 2 &&
+    bool one = w0->prog_running && c->opt_profile.load() < 2 &&
                w0->sends_written + n - __atomic_load_n(&w0->pctl->send_done, __ATOMIC_ACQUIRE) <= SW_SEND_RING;
     for (uint32_t i = 1; one && i < n; i++) one = b.items[i].op->w == w0;
     // the put warp takes a lane per put for RTS descriptors and payloads up to 256 B; larger eager payloads are
@@ -1906,181 +1876,6 @@ bool poll_puts(Ctx* c) {
   return any;
 }
 
-// ============================================================================ progress: matching
-bool pump_match(Ctx* c, Worker* w) {
-  if (w->match_inflight || !w->mstate) return false;
-  int st = w->status.load(std::memory_order_acquire);
-  if (st != SW_ST_RUNNING && st != SW_ST_CLOSING) return false;
-  SwMatchIn* in = w->min;
-  uint32_t np = 0;
-  uint64_t new_arrivals = 0;
-  for (Ep* ep : w->eps) {
-    uint64_t p = ep->in->produced.load(std::memory_order_acquire);
-    in->produced[ep->index] = p;
-    uint64_t consumed = ep->in->consumed.load(std::memory_order_relaxed);
-    if (p > consumed) new_arrivals += p - consumed;
-  }
-  if (w->close_phase == 0) {
-    while (!w->new_posts.empty() && np < SW_MAX_POSTS && w->posted_est + np < SW_PQ_CAP / 2) {
-      RecvOp* r = w->new_posts.front();
-      uint64_t buf = (uint64_t)(uintptr_t)r->ptr;
-      if (r->mem == SW_MEM_HOST && r->cap > HOST_BOUNCE_MAX) {
-        swgpu::PtrInfo pi;
-        swgpu::ptr_info(r->ptr, &pi);
-        if (pi.is_pinned) r->mem = MEM_PINNED;  // the pull kernel writes the caller's pinned buffer directly
-      }
-      if (r->mem == SW_MEM_HOST) {
-        if (r->cap <= HOST_BOUNCE_MAX) {
-          r->pinned_bounce = c->host_pool.get(r->cap);
-          buf = (uint64_t)(uintptr_t)r->pinned_bounce;
-        } else {
-          r->dev_staging = c->staging.get(r->cap, &r->staging_size);
-          buf = (uint64_t)(uintptr_t)r->dev_staging;
-        }
-        if (!buf) {
-          w->new_posts.pop_front();
-          complete(c, w, r->op_id, SW_OP_RECV, SW_ERR_NO_MEMORY);
-          delete r;
-          continue;
-        }
-      }
-      SwPost& p = in->posts[np++];
-      p.tag = r->tag;
-      p.mask = r->mask;
-      p.buf = buf;
-      p.cap = r->cap;
-      p.op_id = r->op_id;
-      w->recvs[r->op_id] = r;
-      w->new_posts.pop_front();
-    }
-  }
-  // arrivals can only make progress when something new happened: new slots, or new
-  // receives that may unblock a ring stalled on the unexpected heap
-  bool stalled_retry = np > 0;
-  uint64_t unseen = 0;
-  for (Ep* ep : w->eps) {
-    uint64_t p = in->produced[ep->index];
-    uint64_t seen = ep->in->consumed.load(std::memory_order_relaxed);
-    if (p > seen) unseen += p - seen;
-  }
-  // a launch that consumed nothing (rings stalled on the unexpected heap) is repeated only when
-  // something changed: new receives, or new slots on any ring
-  if (np == 0 && (unseen == 0 || (w->match_posts_inflight == 0xFFFFFFFFu && !stalled_retry && unseen == w->stall_unseen)))
-    return false;
-  w->stall_unseen = unseen;
-  in->n_posts = np;
-  in->n_eps = (uint32_t)w->eps.size();
-  in->max_arrivals = SW_MAX_ARRIVALS;
-  w->mtimed = c->opt_profile.load() >= 2;
-  if (w->mtimed) swgpu::event_record(w->mev_start, c->s_match);
-  uint32_t max_jobs = np + (uint32_t)std::min<uint64_t>(unseen, SW_MAX_ARRIVALS);
-  trace(c, "match_launch", np, unseen);
-  const SwMatchScalars* sc = nullptr;
-  if (w->eps.size() <= SW_SC_EPS) {
-    for (Ep* ep : w->eps) {
-      w->msc.ring_cons[ep->index] = ep->in->consumed.load(std::memory_order_relaxed);  // == device ring cursor
-      w->msc.ring_base[ep->index] = (uint64_t)(uintptr_t)ep->ring;
-      w->msc.ring_slots[ep->index] = ep->ring_slots;
-    }
-    sc = &w->msc;
-  }
-  swgpu::DoneFlag df{nullptr, ++c->flag_seq};
-  const int lr = swgpu::launch_match_deliver(c->s_match, w->mstate, in, w->mout, max_jobs, sc,
-                                             (w->mtimed || !c->opt_done_flags.load()) ? nullptr : &df);
-  if (lr < 0) fprintf(stderr, "starway_b200: match/deliver launch failed: %s\n", swgpu::last_error());
-  w->mflag_mode = lr == 1;
-  w->mdone_seq = df.value;
-  w->mspins = 0;
-  if (!w->mflag_mode) swgpu::event_record(w->mtimed ? w->mev : w->mev_fast, c->s_match);
-  w->match_inflight = true;
-  w->match_posts_inflight = np;
-  w->posted_est += np;
-  std::lock_guard<std::mutex> lk(c->st_mu);
-  c->stats.match_launches++;
-  c->stats.deliver_launches += max_jobs ? 1 : 0;
-  c->stats.match_posts += np;
-  return true;
-}
-
-bool poll_match(Ctx* c, Worker* w) {
-  if (!w->match_inflight) return false;
-  int q;
-  if (w->mflag_mode) {
-    q = __atomic_load_n(&w->mout->done_seq, __ATOMIC_ACQUIRE) == w->mdone_seq ? 0 : 1;
-    if (q == 1 && (++w->mspins & 0x3FF) == 0 && swgpu::stream_query(c->s_match) < 0) q = -1;
-  } else {
-    q = swgpu::event_query(w->mtimed ? w->mev : w->mev_fast);
-  }
-  if (q == 1) return false;
-  if (q < 0) fprintf(stderr, "starway_b200: match/deliver kernel failed: %s\n", swgpu::last_error());
-  w->match_inflight = false;
-  SwMatchOut* out = w->mout;
-  trace(c, "match_done", out->n_jobs, out->n_rndv);
-  if (w->mtimed) {
-    float ms = swgpu::event_elapsed_ms(w->mev_start, w->mev);
-    if (ms >= 0) {
-      std::lock_guard<std::mutex> lk(c->st_mu);
-      c->stats.match_event_ms += ms;
-      c->stats.match_event_launches++;
-    }
-  }
-  if (out->err) fprintf(stderr, "starway_b200: device matcher reported inconsistency 0x%x\n", out->err);
-  {
-    // keep the ring entries (filled per launch), take the queue cursors the kernel reported
-    SwMatchScalars next = out->sc;
-    memcpy(next.ring_cons, w->msc.ring_cons, sizeof(next.ring_cons));
-    memcpy(next.ring_base, w->msc.ring_base, sizeof(next.ring_base));
-    memcpy(next.ring_slots, w->msc.ring_slots, sizeof(next.ring_slots));
-    next.valid = out->sc.valid;
-    w->msc = next;
-  }
-  // credits first: the slots are free again
-  bool stalled = false;
-  for (Ep* ep : w->eps) {
-    uint64_t cns = out->consumed[ep->index];
-    if (cns != ep->in->consumed.load(std::memory_order_relaxed)) ep->in->consumed.store(cns, std::memory_order_release);
-    if (cns < w->min->produced[ep->index]) stalled = true;
-  }
-  // remember a heap-stall so that we do not spin relaunching until new receives arrive
-  w->match_posts_inflight = (stalled && out->n_arrivals == 0 && w->min->n_posts == 0) ? 0xFFFFFFFFu : 0;
-  {
-    std::lock_guard<std::mutex> lk(c->st_mu);
-    c->stats.match_arrivals += out->n_arrivals;
-  }
-  w->posted_est = out->n_posted;
-  uint32_t nj = std::min<uint32_t>(out->n_jobs, SW_MAX_JOBS);
-  for (uint32_t i = 0; i < nj; i++) {
-    const SwCqe& e = out->cq[i];
-    if (e.kind != SW_JOB_DELIVER) continue;
-    recv_finish(c, w, e.op_id, e.status, e.tag, e.len);
-  }
-  uint32_t nr = std::min<uint32_t>(out->n_rndv, SW_MAX_JOBS);
-  for (uint32_t i = 0; i < nr; i++) {
-    const SwRndvRec& r = out->rndv[i];
-    BulkJob j;
-    j.w = w;
-    j.ep = r.ep < w->eps.size() ? w->eps[r.ep] : nullptr;
-    j.recv_op = r.op_id;
-    j.dst = r.dst;
-    j.cap = r.cap;
-    j.tag = r.tag;
-    j.len = r.len;
-    j.rts = r.rts;
-    j.t_enq = now_s();
-    {
-      auto rit = w->recvs.find(r.op_id);
-      j.src_host = (r.rts.pad[0] & 1) != 0;
-      j.host_side = j.src_host || (rit != w->recvs.end() && rit->second->mem == MEM_PINNED);
-    }
-    if (r.status != SW_OK) {
-      j.failed = true;
-      j.fail_status = r.status;
-    }
-    c->pending_bulk.push_back(j);
-  }
-  return true;
-}
-
 // ============================================================================ progress: rendezvous pulls
 uint64_t pull_outstanding(Ctx* c);
 // device-side users of the mapping table / of mapped addresses: running control kernels, unfinished pulls
@@ -2104,7 +1899,7 @@ void* resolve_mapping(Ctx* c, BulkJob& j, bool* retry) {
     // distinct IPC handles are normal).  Opening/closing a mapping costs ~100s of us, so only
     // the least recently used idle quarter is dropped when the bound is hit.
     if (c->mappings.size() >= (size_t)std::max<int64_t>(1, c->opt_max_mappings.load())) {
-      if (c->map_tbl && mappings_in_use_on_device(c)) {
+      if (mappings_in_use_on_device(c)) {
         // A control kernel may be resolving through the table, a pull may be reading through a mapping:
         // have the control kernels leave (no relaunch while evict_pending), let the pulls drain, come back.
         c->evict_pending = true;
@@ -2125,13 +1920,12 @@ void* resolve_mapping(Ctx* c, BulkJob& j, bool* retry) {
         swgpu::ipc_close(m->second.base);
         c->mappings.erase(m);
       }
-      if (c->map_tbl) {   // rebuild the device table from what is left
-        swgpu::map_table_clear(c->map_tbl);
-        for (auto& kv : c->mappings)
-          if (kv.second.buf_id)
-            swgpu::map_table_insert(c->map_tbl, c->s_map, kv.second.uuid, kv.second.buf_id, kv.second.remote_base,
-                                    (uint64_t)(uintptr_t)kv.second.base);
-      }
+      // rebuild the device table from what is left
+      swgpu::map_table_clear(c->map_tbl);
+      for (auto& kv : c->mappings)
+        if (kv.second.buf_id)
+          swgpu::map_table_insert(c->map_tbl, c->s_map, kv.second.uuid, kv.second.buf_id, kv.second.remote_base,
+                                  (uint64_t)(uintptr_t)kv.second.base);
     }
     void* base = nullptr;
     if (swgpu::ipc_open(j.rts.ipc_handle, &base) != 0) {
@@ -2139,7 +1933,7 @@ void* resolve_mapping(Ctx* c, BulkJob& j, bool* retry) {
       return nullptr;
     }
     Mapping m{base, 0, now_s(), j.rts.ctx_uuid, j.rts.pad[1], j.rts.alloc_base};
-    if (c->map_tbl && m.buf_id &&
+    if (m.buf_id &&
         swgpu::map_table_insert(c->map_tbl, c->s_map, m.uuid, m.buf_id, m.remote_base, (uint64_t)(uintptr_t)base) != 0)
       m.buf_id = 0;   // probe window full: this allocation keeps going through the host
     it = c->mappings.emplace(key, m).first;
@@ -2174,10 +1968,10 @@ bool pump_bulk(Ctx* c) {
   }
   if ((c->bulk_tail - c->bulk_head) >= (uint32_t)N_BULK_BLOCKS) return false;
   {
-    // Coalesce: while more matches are on their way (ops queued, puts or matches in flight), hold the
-    // launch until enough bytes are pending or the oldest job has waited opt_coalesce_us.
+    // Coalesce: while more matches are on their way (ops queued, puts in flight, receives not yet handed to
+    // the device), hold the launch until enough bytes are pending or the oldest job has waited opt_coalesce_us.
     bool upstream = c->sq_head.load(std::memory_order_acquire) != nullptr || c->put_head != c->put_tail;
-    for (Worker* w : c->active) upstream |= w->match_inflight || !w->new_posts.empty();
+    for (Worker* w : c->active) upstream |= !w->new_posts.empty();
     if (upstream) {
       uint64_t bytes = 0;
       for (auto& j : c->pending_bulk) bytes += j.len;
@@ -2359,8 +2153,8 @@ bool poll_bulk(Ctx* c) {
 }
 
 // ============================================================================ progress: resident control kernel
-// Replaces pump_match / poll_match when the worker runs on the resident path: the host only feeds the post
-// ring, drains the completion rings and keeps the kernels alive while work is expected.
+// The host only feeds the post ring, drains the completion rings and keeps the kernels alive while work is
+// expected.
 uint64_t unseen_arrivals(Worker* w) {
   uint64_t unseen = 0;
   for (Ep* ep : w->eps) {
@@ -2624,7 +2418,6 @@ void pull_collect_stats(Ctx* c) {
 }
 
 bool pump_pull(Ctx* c) {
-  if (!c->pq) return false;
   bool any = false;
   if (c->pull_running) {
     if (__atomic_load_n(&c->pull_ctl->exited, __ATOMIC_ACQUIRE) == c->pull_seq && swgpu::event_query(c->pull_ev) != 1) {
@@ -2754,27 +2547,16 @@ bool poll_ctl(Ctx* c, Ep* ep) {
         break;
       case CTL_CANCEL_RTS: {
         // the sender is closing and withdraws rendezvous m.a
+        // The control kernel may match (and the pull CTAs may copy) this request at any moment: raise the
+        // endpoint's dead bit -- matches of its requests then come to the host -- and acknowledge once
+        // the kernel has seen the bit and every pull it issued before that has completed
+        // (progress_cancels).
         Worker* w = ep->owner;
-        if (w->resident) {
-          // The control kernel may match (and the pull CTAs may copy) this request at any moment: raise the
-          // endpoint's dead bit -- matches of its requests then come to the host -- and acknowledge once
-          // the kernel has seen the bit and every pull it issued before that has completed
-          // (progress_cancels).
-          ep->cancel_quiesce.push_back(m.a);
-          __atomic_store_n(&w->pctl->dead_mask, w->pctl->dead_mask | (1ull << (ep->index & 63)), __ATOMIC_RELEASE);
-          __atomic_store_n(&w->pctl->host_epoch, ++w->host_epoch, __ATOMIC_RELEASE);
-          ep->cancel_epoch = w->host_epoch;
-          ep->cancel_pull_mark = ~0ull;
-          break;
-        }
-        bool in_flight = false;
-        for (uint32_t k = c->bulk_head; k != c->bulk_tail; k++)
-          for (BulkJob& j : c->bulk_blocks[k % N_BULK_BLOCKS].jobs)
-            if (j.ep == ep && j.rts.send_seq == m.a) in_flight = true;
-        if (!in_flight) {
-          ep->canceled_rts.insert(m.a);
-          ctl_send(ep, CTL_CANCEL_ACK, SW_OK, m.a);
-        }  // else: the FIN of the running pull acknowledges it
+        ep->cancel_quiesce.push_back(m.a);
+        __atomic_store_n(&w->pctl->dead_mask, w->pctl->dead_mask | (1ull << (ep->index & 63)), __ATOMIC_RELEASE);
+        __atomic_store_n(&w->pctl->host_epoch, ++w->host_epoch, __ATOMIC_RELEASE);
+        ep->cancel_epoch = w->host_epoch;
+        ep->cancel_pull_mark = ~0ull;
         break;
       }
       case CTL_CLOSE:
@@ -2801,7 +2583,7 @@ bool poll_ctl(Ctx* c, Ep* ep) {
 // mapping back; the ring index is reused by a later connection (with a new generation).  The record itself
 // stays listed (reference: list_clients never shrinks, tests/test_basic.py:53-56).
 bool retire_eps(Ctx* c, Worker* w) {
-  if (!w->resident || w->kind != SW_WORKER_SERVER || w->close_phase != 0) return false;
+  if (w->kind != SW_WORKER_SERVER || w->close_phase != 0) return false;
   bool any = false;
   for (Ep* ep : w->eps) {
     if (ep->retired || !ep->peer_closed || ep->close_ack_owed || !ep->shm) continue;
@@ -2837,7 +2619,7 @@ bool retire_eps(Ctx* c, Worker* w) {
   return any;
 }
 
-// resident path: withdrawals wait until the device cannot touch the withdrawn sources any more
+// withdrawals wait until the device cannot touch the withdrawn sources any more
 bool progress_cancels(Ctx* c, Worker* w) {
   bool any = false;
   for (Ep* ep : w->eps) {
@@ -2910,14 +2692,6 @@ void worker_release(Ctx* c, Worker* w, bool leak_rings) {
     swgpu::match_state_destroy(w->mstate);
     w->mstate = nullptr;
   }
-  if (w->min) swgpu::host_free(w->min);
-  if (w->mout) swgpu::host_free(w->mout);
-  w->min = nullptr;
-  w->mout = nullptr;
-  if (w->mev) swgpu::event_destroy(w->mev);
-  if (w->mev_start) swgpu::event_destroy(w->mev_start);
-  if (w->mev_fast) swgpu::event_destroy(w->mev_fast);
-  w->mev = w->mev_start = w->mev_fast = nullptr;
   if (w->s_ctl) {
     swgpu::stream_sync(w->s_ctl);
     swgpu::stream_destroy(w->s_ctl);
@@ -2977,8 +2751,8 @@ bool progress_close(Ctx* c, Worker* w) {
   }
   if (w->close_phase == 2) {
     // ---- wait for in-flight device work and for the cancel acknowledgements
-    bool busy = w->match_inflight || w->bulk_inflight > 0;
-    if (w->resident && w->pctl) {
+    bool busy = w->bulk_inflight > 0;
+    if (w->pctl) {
       // the control kernel is asked to leave (pump_progress raises `stop` from phase 2 on); rendezvous copies
       // it handed to the pull CTAs run to completion -- they write into receive buffers of this worker
       busy |= w->prog_running;
@@ -3219,14 +2993,9 @@ void progress_main(Ctx* c) {
         active |= poll_ctl(c, ep);
         active |= poll_fin_words(c, ep);
       }
-      if (w->resident) {
-        active |= pump_progress(c, w);
-        active |= progress_cancels(c, w);
-        if ((iter & 255) == 0) active |= retire_eps(c, w);
-      } else {
-        active |= poll_match(c, w);
-        active |= pump_match(c, w);
-      }
+      active |= pump_progress(c, w);
+      active |= progress_cancels(c, w);
+      if ((iter & 255) == 0) active |= retire_eps(c, w);
       check_flushes(c, w);
       active |= progress_close(c, w);
       if ((iter & 31) == 0 && w->kind == SW_WORKER_SERVER) poll_listeners(c, w);
@@ -3249,8 +3018,7 @@ void progress_main(Ctx* c) {
     inflight |= c->pull_running;
     bool expecting = false;  // operations whose completion depends on a peer's doorbell / FIN
     for (Worker* w : c->active) {
-      inflight |= w->match_inflight || w->prog_running;
-      resident_only &= !w->match_inflight;
+      inflight |= w->prog_running;
       if (w->close_phase >= 4) continue;
       expecting |= !w->recvs.empty() || !w->flushes.empty() || w->close_phase != 0;
       for (Ep* ep : w->eps) expecting |= !ep->rndv_wait.empty() || !ep->sendq.empty();
@@ -3364,9 +3132,8 @@ sw_ctx* sw_ctx_create(int device) {
   memset(&c->stats, 0, sizeof(c->stats));
   c->efd = eventfd(0, EFD_NONBLOCK | EFD_CLOEXEC);
   c->s_put = swgpu::stream_create();
-  c->s_match = swgpu::stream_create();
   c->s_bulk = swgpu::stream_create();
-  bool ok = c->s_put && c->s_match && c->s_bulk;
+  bool ok = c->s_put && c->s_bulk;
   for (int i = 0; ok && i < N_PUT_BLOCKS; i++) {
     PutBlock& b = c->put_blocks[i];
     b.descs = (SwPutDesc*)swgpu::host_alloc(sizeof(SwPutDesc) * PUT_BATCH);
@@ -3394,9 +3161,9 @@ sw_ctx* sw_ctx_create(int device) {
     delete c;
     return nullptr;
   }
-  // ---- resident path: pull queue, mapping table; needs page-locking of existing host mappings (control blocks)
-  if (const char* e = getenv("STARWAY_RESIDENT")) c->opt_resident = atoll(e);
-  if (c->opt_resident.load()) {
+  // ---- resident path: pull queue, mapping table.  The control kernels publish credits and FIN words through
+  // page-locked aliases of the connections' shared control blocks: check once that such mappings can be locked.
+  {
     void* probe = mmap(nullptr, 4096, PROT_READ | PROT_WRITE, MAP_SHARED | MAP_ANONYMOUS, -1, 0);
     bool can_lock = false;
     if (probe != MAP_FAILED) {
@@ -3405,23 +3172,22 @@ sw_ctx* sw_ctx_create(int device) {
       munmap(probe, 4096);
     }
     if (!can_lock) {
-      fprintf(stderr, "starway_b200: cannot page-lock shared mappings (%s): using host-driven launches\n", swgpu::last_error());
-      c->opt_resident = 0;
-    }
-  }
-  if (c->opt_resident.load()) {
-    c->pq = swgpu::pull_queue_create();
-    c->map_tbl = swgpu::map_table_create();
-    c->pull_ctl = (SwPullCtl*)swgpu::host_alloc(sizeof(SwPullCtl));
-    c->s_pull = swgpu::stream_create();
-    c->s_map = swgpu::stream_create();
-    c->pull_ev = swgpu::event_create(0);
-    c->opt_pull_ctas = swgpu::pull_default_ctas();
-    if (!c->pq || !c->map_tbl || !c->pull_ctl || !c->s_pull || !c->s_map || !c->pull_ev) {
-      set_error(std::string("sw_ctx_create (resident path): ") + swgpu::last_error());
+      set_error(std::string("sw_ctx_create: cannot page-lock shared host mappings: ") + swgpu::last_error());
       delete c;
       return nullptr;
     }
+  }
+  c->pq = swgpu::pull_queue_create();
+  c->map_tbl = swgpu::map_table_create();
+  c->pull_ctl = (SwPullCtl*)swgpu::host_alloc(sizeof(SwPullCtl));
+  c->s_pull = swgpu::stream_create();
+  c->s_map = swgpu::stream_create();
+  c->pull_ev = swgpu::event_create(0);
+  c->opt_pull_ctas = swgpu::pull_default_ctas();
+  if (!c->pq || !c->map_tbl || !c->pull_ctl || !c->s_pull || !c->s_map || !c->pull_ev) {
+    set_error(std::string("sw_ctx_create (resident path): ") + swgpu::last_error());
+    delete c;
+    return nullptr;
   }
   if (const char* e = getenv("STARWAY_COPY_THREADS")) c->opt_copy_threads = std::max<int64_t>(0, atoll(e));
   {
@@ -3549,7 +3315,6 @@ void sw_ctx_destroy(sw_ctx* ctx) {
   c->host_pool.destroy();
   c->staging.destroy();
   swgpu::stream_destroy(c->s_put);
-  swgpu::stream_destroy(c->s_match);
   swgpu::stream_destroy(c->s_bulk);
   if (c->efd >= 0) close(c->efd);
   {
@@ -3591,7 +3356,6 @@ int sw_set_option(sw_ctx* ctx, const char* key, int64_t value) {
   else if (k == "done_flags") c->opt_done_flags = value;
   else if (k == "bulk_balance") c->opt_bulk_balance = value;
   else if (k == "consumer_polling") c->consumer_polling.store(value != 0, std::memory_order_seq_cst);
-  else if (k == "resident") c->opt_resident = (value != 0 && c->pq) ? 1 : 0;   // applies to workers created afterwards
   else if (k == "linger_us") c->opt_linger_us = std::max<int64_t>(1, value);
   else if (k == "max_life_us") c->opt_max_life_us = std::max<int64_t>(10, value);
   else if (k == "armed_ms") c->opt_armed_ms = std::max<int64_t>(0, value);
@@ -3616,7 +3380,7 @@ int64_t sw_get_option(sw_ctx* ctx, const char* key) {
   if (k == "heap_big_blocks") return c->opt_heap_big;
   if (k == "profile") return c->opt_profile;
   if (k == "sm_count") return swgpu::sm_count();
-  if (k == "resident") return c->opt_resident;
+  if (k == "resident") return 1;   // receives always run on the resident control kernels (read-only)
   if (k == "linger_us") return c->opt_linger_us;
   if (k == "max_life_us") return c->opt_max_life_us;
   if (k == "armed_ms") return c->opt_armed_ms;
@@ -3967,10 +3731,9 @@ double sw_evaluate_perf(sw_ctx* ctx, sw_worker_t wid, sw_ep_t epid, size_t msg_s
   Ep* ep = epid ? find_ep(c, epid) : (w->eps.empty() ? nullptr : w->eps[0]);
   const bool same_gpu = !ep || ep->in_process || ep->peer_device == c->device;
   const bool eager = msg_size <= (size_t)c->opt_eager_max.load();
-  // One-way latency through the asyncio API on one GPU: 64 B 29.9 us, 1 MiB 52.3 us (resident=0: 64.3 / 91.5 us).
+  // One-way latency through the asyncio API on one GPU: 64 B 29.9 us, 1 MiB 52.3 us.
   // A peer over NVLink has not been measured on H100; its estimate takes the same latency.
-  const bool resident = c->opt_resident.load() != 0;
-  const double lat = resident ? (eager ? 29.9e-6 : 52.3e-6) : (eager ? 64.3e-6 : 91.5e-6);
+  const double lat = eager ? 29.9e-6 : 52.3e-6;
   // copy rate of one large message: HBM copy on one GPU (1.16 TB/s payload at 1 GiB, measured), NVLink 4 pull
   // between GPUs (450 GB/s per direction, nominal: not measured)
   const double bw = same_gpu ? 1.16e12 : 4.5e11;
@@ -3979,7 +3742,7 @@ double sw_evaluate_perf(sw_ctx* ctx, sw_worker_t wid, sw_ep_t epid, size_t msg_s
 
 int sw_stats_get(sw_ctx* ctx, sw_stats* out) {
   Ctx* c = (Ctx*)ctx;
-  if (c->pq && !tls_is_progress) {
+  if (!tls_is_progress) {
     // the pull CTAs publish their byte / busy-time counters when they leave: ask them to (they are relaunched
     // at once if copies are outstanding), bounded wait
     c->stats_flush.store(1, std::memory_order_release);

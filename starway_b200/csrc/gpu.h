@@ -80,19 +80,13 @@ int match_state_set_ring(SwMatchState* st, uint32_t ep, void* ring_base, uint32_
 // Kernel launches (asynchronous on `s`).
 // Completion flag: a word in pinned host memory that a single-CTA launch stores `value` to (system
 // scope, after all its other stores) so that the host can spin on memory instead of on a CUDA event.
-// launch_put / launch_match_deliver return 1 when the launch will write the flag, 0 when the batch is
-// too large for the flag-writing variant (the caller records an event instead), < 0 on error.
+// launch_put returns 1 when the launch will write the flag, 0 when the batch is too large for the
+// flag-writing variant (the caller records an event instead), < 0 on error.
 struct DoneFlag {
-  volatile uint64_t* flag;   // launch_put only; launch_match_deliver writes SwMatchOut::done_seq
+  volatile uint64_t* flag;
   uint64_t value;            // non-zero
 };
 int launch_put(stream_t s, const SwPutDesc* descs, uint32_t n, const DoneFlag* done = nullptr);
-int launch_match(stream_t s, SwMatchState* st, const SwMatchIn* in, SwMatchOut* out);
-int launch_deliver(stream_t s, SwMatchState* st, SwMatchOut* out, uint32_t max_jobs);
-// match + deliver for one batch: a single fused launch when the batch is small
-// `sc`: the queue cursors reported by the previous launch of this worker (nullptr: read them on the device)
-int launch_match_deliver(stream_t s, SwMatchState* st, const SwMatchIn* in, SwMatchOut* out, uint32_t max_jobs,
-                         const SwMatchScalars* sc, const DoneFlag* done = nullptr);
 int launch_bulk(stream_t s, const SwSeg* segs, uint32_t nseg, const BulkTuning* tune);
 
 // ---------------------------------------------------------------- resident progress path

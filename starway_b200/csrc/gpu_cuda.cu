@@ -343,9 +343,6 @@ SwMatchState* match_state_create(uint32_t heap_small_blocks, uint32_t heap_big_b
   SW_ALLOC(heap_big, uint8_t, (size_t)heap_big_blocks * SW_HEAP_BIG_BYTES);
   SW_ALLOC(free_small, uint32_t, heap_small_blocks);
   SW_ALLOC(free_big, uint32_t, heap_big_blocks);
-  SW_ALLOC(pend_small, uint32_t, heap_small_blocks);
-  SW_ALLOC(pend_big, uint32_t, heap_big_blocks);
-  SW_ALLOC(jobs, SwJob, SW_MAX_JOBS);
 #undef SW_ALLOC
   {
     std::vector<uint32_t> idx(heap_small_blocks > heap_big_blocks ? heap_small_blocks : heap_big_blocks);
@@ -376,9 +373,8 @@ int match_state_destroy(SwMatchState* st) {
   }
   if (!o) return -1;
   SwMatchState& h = o->host;
-  void* ptrs[] = {h.p_tag,  h.p_mask, h.p_buf,      h.p_cap,    h.p_op,     h.p_valid,  h.u_tag,   h.u_len, h.u_data,
-                  h.u_meta, h.u_blk,  h.heap_small, h.heap_big, h.free_small, h.free_big, h.pend_small, h.pend_big,
-                  h.jobs,   o->dev};
+  void* ptrs[] = {h.p_tag,  h.p_mask, h.p_buf,      h.p_cap,    h.p_op,       h.p_valid, h.u_tag, h.u_len, h.u_data,
+                  h.u_meta, h.u_blk,  h.heap_small, h.heap_big, h.free_small, h.free_big, o->dev};
   for (void* p : ptrs) dev_free(p);
   delete o;
   return 0;
@@ -425,54 +421,6 @@ int launch_put(stream_t s, const SwPutDesc* descs, uint32_t n, const DoneFlag* d
   const uint32_t cap = (uint32_t)g_sms * 8;
   if (grid > cap) grid = cap;
   sw_put_kernel<<<grid, warps_per_cta * 32, 0, (cudaStream_t)s>>>(descs, n);
-  SW_CUDA(cudaGetLastError());
-  return 0;
-}
-
-static void fill_match_args(SwMatchArgs& a, const SwMatchIn* in, const SwMatchScalars* sc = nullptr) {
-  if (sc)
-    a.sc = *sc;
-  else
-    memset(&a.sc, 0, sizeof(a.sc));
-  a.n_posts = in->n_posts;
-  a.n_eps = in->n_eps;
-  a.max_arrivals = in->max_arrivals;
-  a.pad = 0;
-  a.done_value = 0;
-  for (uint32_t e = 0; e < SW_INLINE_EPS; e++) a.produced[e] = e < in->n_eps ? in->produced[e] : 0;
-  const uint32_t np = in->n_posts <= SW_INLINE_POSTS ? in->n_posts : 0;
-  for (uint32_t i = 0; i < np; i++) a.posts[i] = in->posts[i];
-}
-
-int launch_match(stream_t s, SwMatchState* st, const SwMatchIn* in, SwMatchOut* out) {
-  SwMatchArgs a;
-  fill_match_args(a, in);
-  sw_match_kernel<<<1, 32, 0, (cudaStream_t)s>>>(st, in, out, a);
-  SW_CUDA(cudaGetLastError());
-  return 0;
-}
-
-int launch_match_deliver(stream_t s, SwMatchState* st, const SwMatchIn* in, SwMatchOut* out, uint32_t max_jobs,
-                         const SwMatchScalars* sc, const DoneFlag* done) {
-  if (max_jobs <= SW_FUSED_MAX_JOBS) {
-    SwMatchArgs a;
-    fill_match_args(a, in, sc);
-    a.done_value = done ? done->value : 0;
-    sw_match_deliver_kernel<<<1, SW_FUSED_THREADS, 0, (cudaStream_t)s>>>(st, in, out, a);
-    SW_CUDA(cudaGetLastError());
-    return done ? 1 : 0;
-  }
-  if (launch_match(s, st, in, out) != 0) return -1;
-  return launch_deliver(s, st, out, max_jobs);
-}
-
-int launch_deliver(stream_t s, SwMatchState* st, SwMatchOut* out, uint32_t max_jobs) {
-  if (!max_jobs) return 0;
-  const uint32_t warps_per_cta = 8;
-  uint32_t grid = (max_jobs + warps_per_cta - 1) / warps_per_cta;
-  const uint32_t cap = (uint32_t)g_sms * 4;
-  if (grid > cap) grid = cap;
-  sw_deliver_kernel<<<grid, warps_per_cta * 32, 0, (cudaStream_t)s>>>(st, out);
   SW_CUDA(cudaGetLastError());
   return 0;
 }

@@ -886,7 +886,8 @@ __device__ __forceinline__ uint32_t sw_res_arrivals(SwMatchState* __restrict__ s
   return used;
 }
 
-// compaction of the queues when tombstones dominate (same procedure as sw_match_body)
+// compaction of a queue when tombstones dominate (more than half its capacity between head and tail): the valid
+// entries move down to the head in their order, the tail follows them and the vacated entries are cleared
 __device__ __forceinline__ void sw_res_compact(SwMatchState* __restrict__ st, SwResCtx& c, const uint32_t lane) {
   const uint64_t PQM = SW_PQ_CAP - 1, UQM = SW_UQ_CAP - 1;
   if (c.p_tail - c.p_head > SW_PQ_CAP / 2) {

@@ -70,11 +70,8 @@ struct SwPutDesc {   // pinned host, read by the put kernel
 };
 static_assert(sizeof(SwPutDesc) == 48, "SwPutDesc layout");
 
-// ---------------------------------------------------------------- match kernel I/O
+// ---------------------------------------------------------------- matching
 constexpr uint32_t SW_MAX_EPS = 64;          // inbound endpoints per worker
-constexpr uint32_t SW_MAX_POSTS = 1024;      // new receives per match launch
-constexpr uint32_t SW_MAX_ARRIVALS = 1024;   // ring slots consumed per match launch
-constexpr uint32_t SW_MAX_JOBS = SW_MAX_POSTS + SW_MAX_ARRIVALS;
 
 // Completion status codes (values mirror the UCX codes the reference forwards
 // through ucs_status_string; see sw_status_string in the C-ABI).
@@ -92,48 +89,7 @@ enum : int32_t {
   SW_ERR_BUSY = -15,
 };
 
-struct SwPost {     // one posted receive (reference ClientRecvArgs/ServerRecvArgs, main.hpp:80-86,234-240)
-  uint64_t tag;
-  uint64_t mask;
-  uint64_t buf;     // device-visible destination
-  uint64_t cap;
-  uint64_t op_id;
-};
-
-struct SwMatchIn {  // pinned host
-  uint32_t n_posts;
-  uint32_t n_eps;
-  uint32_t max_arrivals;   // budget for this launch (<= SW_MAX_ARRIVALS)
-  uint32_t pad;
-  uint64_t produced[SW_MAX_EPS];  // slots produced so far on each inbound ring
-  SwPost posts[SW_MAX_POSTS];
-};
-
-enum : uint32_t {
-  SW_JOB_DELIVER = 1,   // copy into a posted receive buffer and complete it
-  SW_JOB_STASH = 2,     // copy an unexpected eager payload from its slot to the heap
-};
-
-struct SwJob {      // device memory: match kernel -> deliver kernel
-  uint64_t src;
-  uint64_t dst;
-  uint64_t len;     // bytes to copy (0 for truncated / zero-length)
-  uint64_t op_id;   // receive being completed (0 for STASH)
-  uint64_t tag;     // sender tag
-  uint64_t msg_len; // full message length (reported as `length`)
-  int32_t status;
-  uint32_t kind;
-};
-
-struct SwCqe {      // pinned host: deliver kernel -> host
-  uint64_t op_id;
-  uint64_t tag;
-  uint64_t len;
-  int32_t status;
-  uint32_t kind;
-};
-
-struct SwRndvRec {  // pinned host: match kernel -> host (receiver pulls the payload)
+struct SwRndvRec {  // a rendezvous match handed to the host (inside SwHrEnt): the receiver pulls the payload
   uint64_t op_id;
   uint64_t dst;
   uint64_t cap;
@@ -142,39 +98,6 @@ struct SwRndvRec {  // pinned host: match kernel -> host (receiver pulls the pay
   uint32_t ep;
   int32_t status;   // SW_OK or SW_ERR_MESSAGE_TRUNCATED
   SwRts rts;
-};
-
-// Queue cursors of one worker.  The match kernel is the only writer; it reports them after every
-// launch (SwMatchOut::sc) and the host hands them back as kernel parameters for the next launch, so a
-// launch does not start with a chain of dependent global loads.
-constexpr uint32_t SW_SC_EPS = 8;
-struct SwMatchScalars {
-  uint64_t p_head, p_tail, u_head, u_tail;
-  uint32_t p_count, u_count;
-  uint32_t n_free_small, n_free_big, n_pend_small, n_pend_big;
-  uint32_t rr_ep;
-  uint32_t valid;                     // 0: the kernel reads the cursors from SwMatchState
-  uint64_t ring_cons[SW_SC_EPS];
-  uint64_t ring_base[SW_SC_EPS];
-  uint32_t ring_slots[SW_SC_EPS];
-};
-
-struct SwMatchOut {  // pinned host
-  uint32_t n_jobs;
-  uint32_t n_rndv;
-  uint32_t n_posted;      // receives left in the posted queue after this launch
-  uint32_t n_unexp;       // messages left in the unexpected queue
-  uint32_t err;           // device-side consistency errors (bad magic/seq)
-  uint32_t n_arrivals;    // slots consumed by this launch
-  uint32_t heap_small_free;
-  uint32_t heap_big_free;
-  uint64_t consumed[SW_MAX_EPS];  // slots consumed so far on each inbound ring
-  SwMatchScalars sc;              // queue cursors after this launch
-  uint64_t done_seq;              // written last by a fused match+deliver launch (system-scope release):
-                                  // the host spins on it instead of on a CUDA event
-  uint64_t pad_done[7];
-  SwCqe cq[SW_MAX_JOBS];
-  SwRndvRec rndv[SW_MAX_JOBS];
 };
 
 // ---------------------------------------------------------------- device-resident queues
@@ -212,14 +135,11 @@ struct SwMatchState {   // device memory, one per worker
   uint64_t fin_ptr[SW_MAX_EPS];      // resident path: device-visible address of the FIN words of that connection
   uint32_t ring_gen[SW_MAX_EPS];     // generation of the ring index (a retired endpoint's index is reused): travels
                                      // with unexpected rendezvous requests so that a stale one is never pulled
-  // unexpected heap: two size classes, index stacks; frees are deferred one launch
+  // unexpected heap: two size classes, stacks of free block indices.  The control kernel pushes a block back once
+  // nothing reads it any more: at once when the matcher warp has copied the payload or read the rendezvous
+  // descriptor, else when the helper warp that copies the payload has finished.
   uint8_t* heap_small;  uint32_t* free_small;  uint32_t n_free_small;  uint32_t cap_small;
   uint8_t* heap_big;    uint32_t* free_big;    uint32_t n_free_big;    uint32_t cap_big;
-  uint32_t* pend_small; uint32_t n_pend_small;
-  uint32_t* pend_big;   uint32_t n_pend_big;
-  // job list for the deliver kernel
-  SwJob* jobs;
-  uint32_t n_jobs;
   uint32_t rr_ep;        // round-robin start endpoint
   // resident path: cursors that survive from one launch of the control kernel to the next
   uint64_t cq_alloc;       // eager completion records written so far
@@ -240,8 +160,7 @@ constexpr uint32_t SW_EP_IDX_BITS = 6, SW_EP_GEN_MASK = 0x3FFu;
 static_assert(SW_MAX_EPS <= (1u << SW_EP_IDX_BITS), "ring index field");
 
 // ---------------------------------------------------------------- resident progress path
-// The receive side of a worker is driven by a RESIDENT (bounded-lifetime) control kernel instead of
-// one match launch per batch: it polls the slot headers of the inbound rings in device memory
+// The receive side of a worker is driven by a RESIDENT (bounded-lifetime) control kernel: it polls the slot headers of the inbound rings in device memory
 // (release/acquire on the header's sequence word -- no host doorbell on the data path), takes new
 // receives from a ring in pinned host memory, matches, delivers eager payloads, publishes credits and
 // completion records straight to host-visible memory, and hands rendezvous matches to a pool of

@@ -91,8 +91,7 @@ int main(int argc, char** argv) {
     }
     double msgs = (double)window * steps;
     double gbs = msgs * n / best / 1e9;
-    uint64_t launches = s1.put_launches - s0.put_launches + s1.match_launches - s0.match_launches +
-                        s1.deliver_launches - s0.deliver_launches + s1.bulk_tma_launches - s0.bulk_tma_launches +
+    uint64_t launches = s1.put_launches - s0.put_launches + s1.bulk_tma_launches - s0.bulk_tma_launches +
                         s1.bulk_simt_launches - s0.bulk_simt_launches;
     launches += s1.prog_launches - s0.prog_launches + s1.pull_launches - s0.pull_launches;
     const double pb = (double)(s1.pull_batches - s0.pull_batches), pbusy = s1.pull_busy_ms - s0.pull_busy_ms;

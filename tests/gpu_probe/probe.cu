@@ -1,12 +1,12 @@
 // tests/gpu_probe/probe.cu — GPU-side unit tests and micro-benchmarks for the starway_b200
 // kernels (TEST INFRASTRUCTURE).  Needs a GPU (built for sm_90a by `make probe`):
-//   sw_probe correctness           bulk-copy + put/match/deliver parity vs oracle/tagmatch.c
+//   sw_probe correctness           bulk-copy parity (TMA and SIMT kernels, aligned and unaligned segments)
 //   sw_probe bench                 single-GPU bulk copy bandwidth sweep (TMA vs SIMT tunings)
 //   sw_probe peer                  2-GPU in-process peer pull/push bandwidth, cudaMemcpyPeer ceiling
 //   sw_probe ipc                   2-process CUDA-IPC mapping check + pull bandwidth
-//   sw_probe latency               launch + event-poll latency of the small kernels
+//   sw_probe latency               launch + completion-poll latency of the put kernels
 //   sw_probe balance               bulk copy of n x 1 MiB messages: segment-list kernel vs balanced job-range kernel
-//   sw_probe floor                 launch -> completion-seen floor: event vs flag in pinned memory, per-hop cost
+//   sw_probe floor                 launch -> completion-seen floor: event vs flag in pinned memory
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -15,12 +15,10 @@
 #include <unistd.h>
 #include <algorithm>
 #include <chrono>
-#include <map>
 #include <random>
 #include <string>
 #include <vector>
 
-#include "../../oracle/tagmatch.h"
 #include "../../starway_b200/csrc/gpu.h"
 
 using namespace swgpu;
@@ -159,232 +157,6 @@ static void test_bulk_correctness() {
   dev_free(src);
   dev_free(dst);
   stream_destroy(st);
-}
-
-// ------------------------------------------------------------------ put/match/deliver vs oracle
-struct Msg {
-  uint64_t tag, len, seq_id;
-  bool rts;
-  uint64_t src_off;  // eager payload offset in srcpool
-};
-
-static void test_match_random(uint64_t seed, int rounds, uint32_t heap_small, uint32_t heap_big, bool verbose) {
-  std::mt19937_64 rng(seed);
-  stream_t sp = stream_create(), sm = stream_create();
-  const uint32_t NEP = 3, SLOTS = 64;
-  SwMatchState* st = match_state_create(heap_small, heap_big);
-  REQ(st);
-  uint8_t* rings[NEP];
-  for (uint32_t e = 0; e < NEP; e++) {
-    rings[e] = (uint8_t*)dev_alloc((size_t)SLOTS * SW_SLOT_BYTES);
-    REQ(rings[e]);
-    REQ(match_state_set_ring(st, e, rings[e], SLOTS) == 0);
-  }
-  const size_t SRCPOOL = 4u << 20, DSTPOOL = 64u << 20;
-  uint8_t* srcpool = (uint8_t*)dev_alloc(SRCPOOL);
-  uint8_t* dstpool = (uint8_t*)dev_alloc(DSTPOOL);
-  std::vector<uint8_t> hsrc(SRCPOOL), hdst(DSTPOOL), mirror(DSTPOOL, 0xEE);
-  fill_pattern(hsrc, (uint32_t)seed);
-  CK(cudaMemcpy(srcpool, hsrc.data(), SRCPOOL, cudaMemcpyHostToDevice));
-  CK(cudaMemset(dstpool, 0xEE, DSTPOOL));
-  SwPutDesc* descs = (SwPutDesc*)host_alloc(sizeof(SwPutDesc) * 4096);
-  SwRts* rtsbuf = (SwRts*)host_alloc(sizeof(SwRts) * 4096);
-  SwMatchIn* in = (SwMatchIn*)host_alloc(sizeof(SwMatchIn));
-  SwMatchOut* out = (SwMatchOut*)host_alloc(sizeof(SwMatchOut));
-  REQ(descs && rtsbuf && in && out);
-
-  orc_worker* orc = orc_worker_new();
-  std::vector<Msg> fifo[NEP];        // produced but not yet consumed by the matcher
-  uint64_t prod[NEP] = {0, 0, 0}, cons[NEP] = {0, 0, 0};
-  uint64_t next_op = 1, next_seq = 1;
-  size_t dst_bump = 0;
-  std::map<uint64_t, std::pair<uint64_t, uint64_t>> op_buf;  // op -> (offset, cap)
-  static const uint64_t lens[] = {0, 1, 7, 15, 16, 17, 100, 255, 256, 257, 1000, 4096, 8127, 8128};
-  static const uint64_t masks[] = {0, ~0ull, 0xFF, 0xF0, 0xFFFF};
-  size_t total_match = 0, total_rndv = 0, total_trunc = 0, total_blocked = 0;
-
-  for (int round = 0; round < rounds; round++) {
-    // ---- sender side: put new messages
-    uint32_t nd = 0;
-    for (uint32_t e = 0; e < NEP; e++) {
-      uint32_t free_slots = SLOTS - (uint32_t)(prod[e] - cons[e]);
-      uint32_t n = (uint32_t)(rng() % 24);
-      if (rng() % 8 == 0) n = free_slots;  // sometimes fill the ring
-      n = std::min(n, free_slots);
-      for (uint32_t i = 0; i < n; i++) {
-        Msg m;
-        m.tag = 1 + rng() % 5;
-        if (rng() % 16 == 0) m.tag |= 0xABCD00000000ull;
-        m.rts = (rng() % 7 == 0);
-        m.seq_id = next_seq++;
-        SwPutDesc& d = descs[nd];
-        uint64_t slot = prod[e] % SLOTS;
-        d.dst = (uint64_t)(rings[e] + slot * SW_SLOT_BYTES);
-        d.tag = m.tag;
-        d.seq = prod[e] + 1;
-        if (m.rts) {
-          m.len = 1 + rng() % 3000000;
-          m.src_off = 0;
-          SwRts& r = rtsbuf[nd];
-          memset(&r, 0, sizeof(r));
-          for (int k = 0; k < 64; k++) r.ipc_handle[k] = (uint8_t)(m.seq_id * 31 + k);
-          r.send_seq = m.seq_id;
-          r.src_ptr = 0x1000 + m.seq_id;
-          d.src = (uint64_t)&r;
-          d.len = sizeof(SwRts);
-          d.kind = SW_KIND_RTS;
-        } else {
-          m.len = lens[rng() % (sizeof(lens) / sizeof(lens[0]))];
-          m.src_off = rng() % (SRCPOOL - 8200);
-          if (rng() % 2) m.src_off &= ~15ull;
-          d.src = (uint64_t)(srcpool + m.src_off);
-          d.len = (uint32_t)m.len;
-          d.kind = SW_KIND_EAGER;
-        }
-        d.msg_len = m.len;
-        nd++;
-        prod[e]++;
-        fifo[e].push_back(m);
-      }
-    }
-    REQ(launch_put(sp, descs, nd) == 0);
-    REQ(stream_sync(sp) == 0);
-
-    // ---- receiver side: new posts + arrivals
-    uint32_t np = (uint32_t)(rng() % 48);
-    if (rng() % 5 == 0) np = 0;
-    std::vector<SwPost> posts;
-    for (uint32_t i = 0; i < np; i++) {
-      SwPost p;
-      p.tag = 1 + rng() % 5;
-      p.mask = masks[rng() % 5];
-      static const uint64_t caps[] = {0, 8, 64, 300, 8128, 100000, 4000000};
-      p.cap = caps[rng() % 7];
-      uint64_t room = std::min<uint64_t>(p.cap, 8192);  // eager never writes more than 8128 B
-      dst_bump = (dst_bump + 15) & ~15ull;
-      if (rng() % 3 == 0) dst_bump += rng() % 16;  // misaligned destinations
-      if (dst_bump + room + 64 > DSTPOOL) break;
-      p.buf = (uint64_t)(dstpool + dst_bump);
-      p.op_id = next_op++;
-      op_buf[p.op_id] = {dst_bump, p.cap};
-      dst_bump += room;
-      posts.push_back(p);
-    }
-    in->n_posts = (uint32_t)posts.size();
-    in->n_eps = NEP;
-    in->max_arrivals = (rng() % 6 == 0) ? (uint32_t)(1 + rng() % 40) : SW_MAX_ARRIVALS;
-    for (uint32_t e = 0; e < NEP; e++) in->produced[e] = prod[e];
-    for (size_t i = 0; i < posts.size(); i++) in->posts[i] = posts[i];
-    memset(out, 0xCD, offsetof(SwMatchOut, cq));
-    REQ(launch_match(sm, st, in, out) == 0);
-    REQ(launch_deliver(sm, st, out, SW_MAX_JOBS) == 0);
-    REQ(stream_sync(sm) == 0);
-    REQ(out->err == 0);
-
-    // ---- oracle, same serialisation: posts in order, then rings round-robin from (round % NEP)
-    std::map<uint64_t, orc_match> want;
-    for (auto& p : posts) {
-      orc_match m;
-      auto ob = op_buf[p.op_id];
-      if (orc_post_recv(orc, p.op_id, p.tag, p.mask, mirror.data() + ob.first, p.cap, &m)) want[m.op_id] = m;
-    }
-    for (uint32_t k = 0; k < NEP; k++) {
-      uint32_t e = (uint32_t)((round + k) % NEP);
-      uint64_t c = out->consumed[e];
-      REQ(c >= cons[e] && c <= prod[e]);
-      if (c < prod[e]) total_blocked++;
-      uint64_t n = c - cons[e];
-      for (uint64_t i = 0; i < n; i++) {
-        Msg m = fifo[e].front();
-        fifo[e].erase(fifo[e].begin());
-        orc_match om;
-        if (orc_arrive(orc, e, m.tag, m.rts ? nullptr : hsrc.data() + m.src_off, m.len, m.rts ? m.seq_id : 0, &om))
-          want[om.op_id] = om;
-      }
-      cons[e] = c;
-    }
-    // ---- compare completions
-    std::map<uint64_t, orc_match> got;
-    REQ(out->n_jobs <= SW_MAX_JOBS && out->n_rndv <= SW_MAX_JOBS);
-    for (uint32_t i = 0; i < out->n_jobs; i++) {
-      const SwCqe& c = out->cq[i];
-      if (c.kind != SW_JOB_DELIVER) {
-        REQ(c.kind == SW_JOB_STASH && c.op_id == 0);
-        continue;
-      }
-      orc_match m;
-      memset(&m, 0, sizeof(m));
-      m.op_id = c.op_id;
-      m.sender_tag = c.tag;
-      m.length = c.len;
-      m.status = c.status;
-      REQ(!got.count(m.op_id));
-      got[m.op_id] = m;
-    }
-    for (uint32_t i = 0; i < out->n_rndv; i++) {
-      const SwRndvRec& r = out->rndv[i];
-      orc_match m;
-      memset(&m, 0, sizeof(m));
-      m.op_id = r.op_id;
-      m.sender_tag = r.tag;
-      m.length = r.len;
-      m.status = r.status;
-      m.user = r.rts.send_seq;
-      m.ep = r.ep;
-      REQ(r.rts.src_ptr == 0x1000 + r.rts.send_seq);
-      for (int k = 0; k < 64; k++) REQ(r.rts.ipc_handle[k] == (uint8_t)(r.rts.send_seq * 31 + k));
-      auto ob = op_buf[r.op_id];
-      REQ(r.dst == (uint64_t)(dstpool + ob.first) && r.cap == ob.second);
-      REQ(!got.count(m.op_id));
-      got[m.op_id] = m;
-      total_rndv++;
-    }
-    if (got.size() != want.size()) {
-      fprintf(stderr, "round %d: got %zu completions, oracle %zu\n", round, got.size(), want.size());
-      exit(5);
-    }
-    for (auto& kv : want) {
-      auto it = got.find(kv.first);
-      REQ(it != got.end());
-      const orc_match &a = it->second, &b = kv.second;
-      if (a.sender_tag != b.sender_tag || a.length != b.length || a.status != b.status || a.user != b.user ||
-          (b.user && a.ep != b.ep)) {
-        fprintf(stderr, "round %d op %llu: got tag=%llx len=%llu st=%d user=%llu ep=%u; oracle tag=%llx len=%llu st=%d user=%llu ep=%u\n",
-                round, (unsigned long long)kv.first, (unsigned long long)a.sender_tag, (unsigned long long)a.length,
-                a.status, (unsigned long long)a.user, a.ep, (unsigned long long)b.sender_tag,
-                (unsigned long long)b.length, b.status, (unsigned long long)b.user, b.ep);
-        exit(6);
-      }
-      if (b.status != 0) total_trunc++;
-      total_match++;
-    }
-    REQ(out->n_posted == orc_num_posted(orc));
-    REQ(out->n_unexp == orc_num_unexpected(orc));
-    if (verbose && round % 50 == 0)
-      printf("  round %d: posted=%u unexp=%u heap_small_free=%u heap_big_free=%u\n", round, out->n_posted,
-             out->n_unexp, out->heap_small_free, out->heap_big_free);
-    if (dst_bump > DSTPOOL - (1u << 20)) break;
-  }
-  CK(cudaMemcpy(hdst.data(), dstpool, DSTPOOL, cudaMemcpyDeviceToHost));
-  if (memcmp(hdst.data(), mirror.data(), DSTPOOL) != 0) {
-    size_t i = 0;
-    while (hdst[i] == mirror[i]) i++;
-    fprintf(stderr, "payload mismatch at dstpool byte %zu (got %02x want %02x)\n", i, hdst[i], mirror[i]);
-    exit(7);
-  }
-  printf("[match] seed %llu heap(%u,%u): %zu completions (%zu rndv, %zu truncated, %zu blocked rings) bit-exact vs oracle\n",
-         (unsigned long long)seed, heap_small, heap_big, total_match, total_rndv, total_trunc, total_blocked);
-  orc_worker_free(orc);
-  for (uint32_t e = 0; e < NEP; e++) dev_free(rings[e]);
-  dev_free(srcpool);
-  dev_free(dstpool);
-  host_free(descs);
-  host_free(rtsbuf);
-  host_free(in);
-  host_free(out);
-  match_state_destroy(st);
-  stream_destroy(sp);
-  stream_destroy(sm);
 }
 
 // ------------------------------------------------------------------ benchmarks
@@ -538,74 +310,6 @@ static void bench_latency(FILE* json) {
         if (json)
           fprintf(json, "{\"bench\":\"put_latency_flag\",\"n\":%d,\"len\":%d,\"us\":%.2f}\n", n, len, bestf * 1e6);
       }
-    }
-  }
-  // match+deliver on a FIFO workload
-  SwMatchState* ms = match_state_create(4096, 512);
-  match_state_set_ring(ms, 0, ring, 1024);
-  SwMatchIn* in = (SwMatchIn*)host_alloc(sizeof(SwMatchIn));
-  SwMatchOut* out = (SwMatchOut*)host_alloc(sizeof(SwMatchOut));
-  uint8_t* dst = (uint8_t*)dev_alloc(1024 * 8192);
-  uint64_t prod = 0, op = 1;
-  for (int n : {1, 64, 1024}) {
-    double best = 1e9;
-    event_t ev = event_create(0);
-    for (int it = 0; it < 30; it++) {
-      for (int i = 0; i < n; i++) {
-        descs[i].src = (uint64_t)src;
-        descs[i].dst = (uint64_t)(ring + (size_t)((prod + i) % 1024) * SW_SLOT_BYTES);
-        descs[i].tag = 1;
-        descs[i].seq = prod + i + 1;
-        descs[i].len = 64;
-        descs[i].kind = SW_KIND_EAGER;
-        descs[i].msg_len = 64;
-      }
-      launch_put(st, descs, n);
-      stream_sync(st);
-      prod += n;
-      in->n_posts = n;
-      in->n_eps = 1;
-      in->max_arrivals = SW_MAX_ARRIVALS;
-      in->produced[0] = prod;
-      for (int i = 0; i < n; i++) in->posts[i] = SwPost{1, 0xFFFF, (uint64_t)(dst + (size_t)i * 8192), 8192, op++};
-      double t0 = now_s();
-      launch_match(st, ms, in, out);
-      launch_deliver(st, ms, out, 2 * n);
-      event_record(ev, st);
-      while (event_query(ev) == 1) {
-      }
-      double t1 = now_s();
-      REQ(out->err == 0 && out->n_jobs == (uint32_t)n);
-      if (it > 3) best = std::min(best, t1 - t0);
-    }
-    printf("[latency] match+deliver n=%4d x 64B: %.2f us (%.2f Mmsg/s)\n", n, best * 1e6, n / best / 1e6);
-    if (json) fprintf(json, "{\"bench\":\"match_deliver_latency\",\"n\":%d,\"us\":%.2f}\n", n, best * 1e6);
-    event_destroy(ev);
-    if (2 * n <= 192) {   // fused single-CTA launch, completion flag in SwMatchOut::done_seq
-      static uint64_t seq = 0;
-      double bestf = 1e9;
-      for (int it = 0; it < 30; it++) {
-        for (int i = 0; i < n; i++) {
-          descs[i].dst = (uint64_t)(ring + (size_t)((prod + i) % 1024) * SW_SLOT_BYTES);
-          descs[i].seq = prod + i + 1;
-        }
-        launch_put(st, descs, n);
-        stream_sync(st);
-        prod += n;
-        in->n_posts = n;
-        in->produced[0] = prod;
-        for (int i = 0; i < n; i++) in->posts[i] = SwPost{1, 0xFFFF, (uint64_t)(dst + (size_t)i * 8192), 8192, op++};
-        DoneFlag df{nullptr, ++seq};
-        double t0 = now_s();
-        REQ(launch_match_deliver(st, ms, in, out, 2 * n, nullptr, &df) == 1);
-        while (*(volatile uint64_t*)&out->done_seq != seq) {
-        }
-        double t1 = now_s();
-        REQ(out->err == 0 && out->n_jobs == (uint32_t)n);
-        if (it > 3) bestf = std::min(bestf, t1 - t0);
-      }
-      printf("[latency] fused match+deliver n=%4d x 64B: launch+flag %.2f us\n", n, bestf * 1e6);
-      if (json) fprintf(json, "{\"bench\":\"match_deliver_latency_flag\",\"n\":%d,\"us\":%.2f}\n", n, bestf * 1e6);
     }
   }
 }
@@ -974,28 +678,10 @@ static void bench_balance(FILE* json) {
 
 // ------------------------------------------------------------------ launch/completion floor
 // What one launch -> "host knows it finished" costs on this box, by completion mechanism.
-struct FloorArgs {
-  volatile uint64_t* flag;
-  uint64_t value;
-  const uint64_t* chain;   // pointer-chasing array in device memory
-  uint32_t hops;
-  uint32_t pad;
-  uint8_t ballast[1536];   // the match launch carries ~1.5 KiB of parameters
-};
 __global__ void floor_empty_kernel() {}
 __global__ void floor_flag_kernel(volatile uint64_t* flag, uint64_t value) {
   __threadfence_system();
   *flag = value;
-}
-__global__ void __launch_bounds__(512) floor_cta_flag_kernel(const __grid_constant__ FloorArgs a) {
-  uint64_t idx = threadIdx.x & 7;
-  if (threadIdx.x < 32)
-    for (uint32_t h = 0; h < a.hops; h++) idx = a.chain[idx];   // dependent global loads
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence_system();
-    *a.flag = a.value + (idx & 0);
-  }
 }
 
 static double median(std::vector<double>& v) {
@@ -1009,16 +695,6 @@ static void bench_floor(FILE* json) {
   uint64_t* flag;
   CK(cudaHostAlloc((void**)&flag, 64, cudaHostAllocPortable | cudaHostAllocMapped));
   *flag = 0;
-  uint64_t* chain;
-  {
-    // scattered chain over 64 MiB so that hops miss L2 lines of each other (but may hit L2 when re-run)
-    const size_t n = (64u << 20) / 8;
-    std::vector<uint64_t> h(n);
-    std::mt19937_64 rng(1);
-    for (size_t i = 0; i < n; i++) h[i] = rng() % n;
-    CK(cudaMalloc((void**)&chain, n * 8));
-    CK(cudaMemcpy(chain, h.data(), n * 8, cudaMemcpyHostToDevice));
-  }
   const int iters = 400;
   auto report = [&](const char* name, std::vector<double>& total, std::vector<double>* api = nullptr) {
     const double m = median(total) * 1e6;
@@ -1069,58 +745,8 @@ static void bench_floor(FILE* json) {
     }
     report("flag kernel (fence.sys + store to pinned host), host spins on the flag", tot, &api);
   }
-  for (uint32_t hops : {0u, 1u, 3u, 6u, 12u}) {
-    static FloorArgs a;
-    a.flag = flag;
-    a.chain = chain;
-    a.hops = hops;
-    std::vector<double> tot, api;
-    for (int i = 0; i < iters; i++) {
-      a.value = ++seq;
-      const double t0 = now_s();
-      floor_cta_flag_kernel<<<1, 512, 0, st>>>(a);
-      const double t1 = now_s();
-      while (*(volatile uint64_t*)flag != seq) {
-      }
-      const double t2 = now_s();
-      if (i >= 20) {
-        tot.push_back(t2 - t0);
-        api.push_back(t1 - t0);
-      }
-    }
-    char name[96];
-    snprintf(name, sizeof name, "512-thread CTA, 1.5 KiB params, %2u dependent loads, flag", hops);
-    report(name, tot, &api);
-  }
-  {
-    // same with an event recorded behind it (what the engine did before flags)
-    static FloorArgs a;
-    a.flag = flag;
-    a.chain = chain;
-    a.hops = 3;
-    cudaEvent_t ev;
-    CK(cudaEventCreateWithFlags(&ev, cudaEventDefault));
-    std::vector<double> tot, api;
-    for (int i = 0; i < iters; i++) {
-      a.value = ++seq;
-      const double t0 = now_s();
-      floor_cta_flag_kernel<<<1, 512, 0, st>>>(a);
-      CK(cudaEventRecord(ev, st));
-      const double t1 = now_s();
-      while (cudaEventQuery(ev) == cudaErrorNotReady) {
-      }
-      const double t2 = now_s();
-      if (i >= 20) {
-        tot.push_back(t2 - t0);
-        api.push_back(t1 - t0);
-      }
-    }
-    report("512-thread CTA, 1.5 KiB params,  3 dependent loads, timing event", tot, &api);
-    CK(cudaEventDestroy(ev));
-  }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(st));
-  CK(cudaFree(chain));
   CK(cudaFreeHost(flag));
   CK(cudaStreamDestroy(st));
 }
@@ -1305,14 +931,7 @@ int main(int argc, char** argv) {
   printf("backend %s, %d device(s), %d SMs\n", backend_name(), device_count(), sm_count());
   FILE* json = nullptr;
   if (argc > 2 && strcmp(argv[2], "-") != 0) json = fopen(argv[2], "a");
-  if (cmd == "correctness" || cmd == "all") {
-    test_bulk_correctness();
-    test_match_random(1, 300, 4096, 512, true);
-    test_match_random(2, 300, 4096, 512, false);
-    test_match_random(3, 300, 24, 6, false);   // tiny heap: exercises back-pressure
-    test_match_random(4, 200, 8, 2, false);
-    for (uint64_t s = 10; s < 20; s++) test_match_random(s, 150, 512, 64, false);
-  }
+  if (cmd == "correctness" || cmd == "all") test_bulk_correctness();
   if (cmd == "latency" || cmd == "all") bench_latency(json);
   if (cmd == "bench" || cmd == "all") bench_single(json);
   if (cmd == "floor") bench_floor(json);

@@ -249,20 +249,16 @@ SwMatchState* match_state_create(uint32_t hs, uint32_t hb) {
   st->heap_big = (uint8_t*)calloc((size_t)hb, SW_HEAP_BIG_BYTES);
   st->free_small = (uint32_t*)calloc(hs, 4);
   st->free_big = (uint32_t*)calloc(hb, 4);
-  st->pend_small = (uint32_t*)calloc(hs, 4);
-  st->pend_big = (uint32_t*)calloc(hb, 4);
   for (uint32_t i = 0; i < hs; i++) st->free_small[i] = i;
   for (uint32_t i = 0; i < hb; i++) st->free_big[i] = i;
   st->n_free_small = hs;
   st->n_free_big = hb;
-  st->jobs = (SwJob*)calloc(SW_MAX_JOBS, sizeof(SwJob));
   return st;
 }
 int match_state_destroy(SwMatchState* st) {
   if (!st) return -1;
   void* ptrs[] = {st->p_tag, st->p_mask, st->p_buf, st->p_cap, st->p_op, st->p_valid, st->u_tag, st->u_len, st->u_data,
-                  st->u_meta, st->u_blk, st->heap_small, st->heap_big, st->free_small, st->free_big, st->pend_small,
-                  st->pend_big, st->jobs};
+                  st->u_meta, st->u_blk, st->heap_small, st->heap_big, st->free_small, st->free_big};
   for (void* p : ptrs) free(p);
   free(st);
   return 0;
@@ -300,176 +296,6 @@ int launch_put(stream_t, const SwPutDesc* descs, uint32_t n, const DoneFlag* don
   for (uint32_t i = 0; i < n; i++) n_rts += descs[i].kind == SW_KIND_RTS;
   if (done && n <= 32 && n_rts <= 16) {
     __atomic_store_n((uint64_t*)done->flag, done->value, __ATOMIC_RELEASE);
-    return 1;
-  }
-  return 0;
-}
-
-static void emit_job(SwMatchState* st, uint64_t src, uint64_t dst, uint64_t len, uint64_t op, uint64_t tag,
-                     uint64_t msg_len, int32_t status, uint32_t kind) {
-  SwJob& j = st->jobs[st->n_jobs++];
-  j.src = src;
-  j.dst = dst;
-  j.len = len;
-  j.op_id = op;
-  j.tag = tag;
-  j.msg_len = msg_len;
-  j.status = status;
-  j.kind = kind;
-}
-static void emit_match(SwMatchState* st, SwMatchOut* out, bool is_rts, uint64_t payload, uint64_t stag,
-                       uint64_t msg_len, uint32_t ep, uint64_t buf, uint64_t cap, uint64_t op) {
-  const bool trunc = msg_len > cap;
-  if (!is_rts) {
-    emit_job(st, payload, buf, trunc ? 0 : msg_len, op, stag, msg_len, trunc ? SW_ERR_MESSAGE_TRUNCATED : SW_OK,
-             SW_JOB_DELIVER);
-  } else {
-    SwRndvRec& r = out->rndv[out->n_rndv++];
-    memcpy(&r.rts, (const void*)(uintptr_t)payload, sizeof(SwRts));
-    r.op_id = op;
-    r.dst = buf;
-    r.cap = cap;
-    r.tag = stag;
-    r.len = msg_len;
-    r.ep = ep;
-    r.status = trunc ? SW_ERR_MESSAGE_TRUNCATED : SW_OK;
-  }
-}
-
-int launch_match(stream_t, SwMatchState* st, const SwMatchIn* in, SwMatchOut* out) {
-  const uint64_t PQM = SW_PQ_CAP - 1, UQM = SW_UQ_CAP - 1;
-  st->n_jobs = 0;
-  out->n_rndv = 0;
-  out->err = 0;
-  // deferred frees become allocatable
-  for (uint32_t i = 0; i < st->n_pend_small; i++) st->free_small[st->n_free_small++] = st->pend_small[i];
-  for (uint32_t i = 0; i < st->n_pend_big; i++) st->free_big[st->n_free_big++] = st->pend_big[i];
-  st->n_pend_small = st->n_pend_big = 0;
-  // phase 1: new receives against the unexpected queue (earliest-arrived first)
-  for (uint32_t i = 0; i < in->n_posts; i++) {
-    const SwPost& p = in->posts[i];
-    bool found = false;
-    for (uint64_t idx = st->u_head; idx < st->u_tail; idx++) {
-      uint64_t s = idx & UQM;
-      uint32_t meta = st->u_meta[s];
-      if (!(meta & SW_UMETA_VALID) || !sw_tag_match(st->u_tag[s], p.tag, p.mask)) continue;
-      st->u_meta[s] = 0;
-      st->u_count--;
-      emit_match(st, out, (meta & SW_UMETA_RTS) != 0, st->u_data[s], st->u_tag[s], st->u_len[s],
-                 meta & SW_UMETA_EPMASK, p.buf, p.cap, p.op_id);
-      if (meta & SW_UMETA_BIG)
-        st->pend_big[st->n_pend_big++] = st->u_blk[s];
-      else
-        st->pend_small[st->n_pend_small++] = st->u_blk[s];
-      found = true;
-      break;
-    }
-    while (st->u_head < st->u_tail && !(st->u_meta[st->u_head & UQM] & SW_UMETA_VALID)) st->u_head++;
-    if (!found) {
-      uint64_t s = st->p_tail & PQM;
-      st->p_tag[s] = p.tag;
-      st->p_mask[s] = p.mask;
-      st->p_buf[s] = p.buf;
-      st->p_cap[s] = p.cap;
-      st->p_op[s] = p.op_id;
-      st->p_valid[s] = 1;
-      st->p_tail++;
-      st->p_count++;
-    }
-  }
-  // phase 2: arrivals against the posted queue (earliest-posted first), rings round-robin
-  uint32_t budget = in->max_arrivals < SW_MAX_ARRIVALS ? in->max_arrivals : SW_MAX_ARRIVALS;
-  uint32_t total = 0;
-  const uint32_t n_eps = in->n_eps;
-  const uint32_t rr = n_eps ? st->rr_ep % n_eps : 0;
-  for (uint32_t e = 0; e < n_eps; e++) {
-    const uint32_t ep = (rr + e) % n_eps;
-    uint64_t cons = st->ring_cons[ep];
-    const uint64_t prod = in->produced[ep];
-    while (cons < prod && budget > 0) {
-      const uint8_t* slot = (const uint8_t*)(uintptr_t)(st->ring_base[ep] + (cons & (st->ring_slots[ep] - 1)) * SW_SLOT_BYTES);
-      SwSlotHdr h;
-      memcpy(&h, slot, 32);
-      if (h.magic != SW_SLOT_MAGIC || h.seq != cons + 1) out->err |= 1;
-      const bool is_rts = h.kind == SW_KIND_RTS;
-      const uint64_t payload = (uint64_t)(uintptr_t)(slot + SW_SLOT_HDR);
-      bool found = false;
-      for (uint64_t idx = st->p_head; idx < st->p_tail; idx++) {
-        uint64_t s = idx & PQM;
-        if (!st->p_valid[s] || !sw_tag_match(h.tag, st->p_tag[s], st->p_mask[s])) continue;
-        st->p_valid[s] = 0;
-        st->p_count--;
-        emit_match(st, out, is_rts, payload, h.tag, h.len, ep, st->p_buf[s], st->p_cap[s], st->p_op[s]);
-        found = true;
-        break;
-      }
-      while (st->p_head < st->p_tail && !st->p_valid[st->p_head & PQM]) st->p_head++;
-      if (!found) {
-        const uint64_t need = is_rts ? sizeof(SwRts) : h.len;
-        const bool big = need > SW_HEAP_SMALL_BYTES;
-        if ((big ? st->n_free_big : st->n_free_small) == 0 || st->u_tail - st->u_head >= SW_UQ_CAP) break;
-        uint32_t blk = big ? st->free_big[--st->n_free_big] : st->free_small[--st->n_free_small];
-        uint64_t haddr = big ? (uint64_t)(uintptr_t)st->heap_big + (uint64_t)blk * SW_HEAP_BIG_BYTES
-                             : (uint64_t)(uintptr_t)st->heap_small + (uint64_t)blk * SW_HEAP_SMALL_BYTES;
-        emit_job(st, payload, haddr, need, 0, h.tag, h.len, SW_OK, SW_JOB_STASH);
-        uint64_t s = st->u_tail & UQM;
-        st->u_tag[s] = h.tag;
-        st->u_len[s] = h.len;
-        st->u_data[s] = haddr;
-        st->u_blk[s] = blk;
-        st->u_meta[s] = SW_UMETA_VALID | (big ? SW_UMETA_BIG : 0) | (is_rts ? SW_UMETA_RTS : 0) | (ep & SW_UMETA_EPMASK);
-        st->u_tail++;
-        st->u_count++;
-      }
-      cons++;
-      budget--;
-      total++;
-    }
-    st->ring_cons[ep] = cons;
-    out->consumed[ep] = cons;
-  }
-  st->rr_ep = rr + 1;
-  out->n_arrivals = total;
-  out->n_jobs = st->n_jobs;
-  out->n_posted = st->p_count;
-  out->n_unexp = st->u_count;
-  out->heap_small_free = st->n_free_small;
-  out->heap_big_free = st->n_free_big;
-  out->sc.p_head = st->p_head;
-  out->sc.p_tail = st->p_tail;
-  out->sc.u_head = st->u_head;
-  out->sc.u_tail = st->u_tail;
-  out->sc.p_count = st->p_count;
-  out->sc.u_count = st->u_count;
-  out->sc.n_free_small = st->n_free_small;
-  out->sc.n_free_big = st->n_free_big;
-  out->sc.n_pend_small = st->n_pend_small;
-  out->sc.n_pend_big = st->n_pend_big;
-  out->sc.rr_ep = st->rr_ep;
-  out->sc.valid = 1;
-  return 0;
-}
-
-int launch_deliver(stream_t, SwMatchState* st, SwMatchOut* out, uint32_t) {
-  for (uint32_t i = 0; i < st->n_jobs; i++) {
-    const SwJob& j = st->jobs[i];
-    if (j.len) memcpy((void*)(uintptr_t)j.dst, (const void*)(uintptr_t)j.src, j.len);
-    SwCqe& c = out->cq[i];
-    c.op_id = j.op_id;
-    c.tag = j.tag;
-    c.len = j.msg_len;
-    c.status = j.status;
-    c.kind = j.kind;
-  }
-  return 0;
-}
-
-int launch_match_deliver(stream_t s, SwMatchState* st, const SwMatchIn* in, SwMatchOut* out, uint32_t max_jobs,
-                         const SwMatchScalars*, const DoneFlag* done) {
-  launch_match(s, st, in, out);
-  if (launch_deliver(s, st, out, max_jobs) != 0) return -1;
-  if (done && max_jobs <= 192) {   // the fused single-CTA launch of the CUDA backend
-    __atomic_store_n(&out->done_seq, done->value, __ATOMIC_RELEASE);
     return 1;
   }
   return 0;

@@ -423,8 +423,8 @@ def test_c_abi_direct_device_pointers(cuda_api, port):
     assert torch.equal(dst, src)
     st = ctx.stats()
     # the product kernels moved the data: puts (launched or executed by the resident control kernel), the
-    # control kernel (or, with resident=0, match launches), rendezvous copies by the pull CTAs or a bulk launch
-    assert st["put_launches"] + st["put_resident"] > 0 and st["prog_launches"] + st["match_launches"] > 0
+    # control kernel, rendezvous copies by the pull CTAs or a bulk launch
+    assert st["put_launches"] + st["put_resident"] > 0 and st["prog_launches"] > 0
     assert st["pull_jobs"] + st["bulk_tma_launches"] > 0
 
 
@@ -488,7 +488,7 @@ def test_storm_small_messages_fast_path(cuda_api, port):
 @pytest.mark.parametrize("opts", [{"done_flags": 0}, {"profile": 2}, {"profile": 1}],
                          ids=["events_only", "timed_events", "bulk_timing"])
 def test_completion_detection_modes(cuda_api, port, opts):
-    """Small put / match launches announce completion through a flag in pinned host memory by
+    """Small put launches announce completion through a flag in pinned host memory by
     default; the event-based paths (flags disabled, per-kernel timing) must deliver the same
     results on the oracle-checked random schedule and on device-buffer chaos."""
     ctx = cuda_api.get_context()
