@@ -63,10 +63,14 @@ build/gpu_sim.o: tests/hostsim/gpu_sim.cpp $(CSRC)/gpu.h $(CSRC)/sw_device.h $(C
 	@mkdir -p build
 	$(CXX) $(CXXFLAGS) -c $< -o $@
 
+build/reduce_sim.o: tests/hostsim/reduce_sim.cpp $(CSRC)/gpu.h $(CSRC)/sw_device.h
+	@mkdir -p build
+	$(CXX) $(CXXFLAGS) -c $< -o $@
+
 # Host-logic simulator: the SAME engine.cpp linked against a CPU stand-in for the device
 # backend, used only by `pytest -m "not gpu"` to exercise connection/protocol/flush/close
 # logic (world_size 2 on CPU).  Never loaded by the starway_b200 package.
-$(HOSTSIM): build/engine_sim.o build/gpu_sim.o build/tagmatch.o
+$(HOSTSIM): build/engine_sim.o build/gpu_sim.o build/reduce_sim.o build/tagmatch.o
 	$(CXX) -shared -Wl,-Bsymbolic -Wl,--version-script=tests/hostsim/exports_sim.map -o $@ $^ -lpthread -lrt -ldl
 
 $(PROBE): tests/gpu_probe/probe.cu build/gpu_cuda.o
@@ -88,6 +92,6 @@ hostsim-asan hostsim-tsan: hostsim-%:
 	@mkdir -p build/$*
 	$(SAN_CXX) -O1 -g -fsanitize=$(if $(filter asan,$*),address,thread) -fno-omit-frame-pointer -std=c++17 -fPIC -pthread -Iinclude \
 	  -shared -Wl,-Bsymbolic -Wl,--version-script=tests/hostsim/exports_sim.map -o build/$*/libstarway_hostsim.so \
-	  $(CSRC)/engine.cpp tests/hostsim/gpu_sim.cpp -x c oracle/tagmatch.c -lpthread -lrt -ldl
+	  $(CSRC)/engine.cpp tests/hostsim/gpu_sim.cpp tests/hostsim/reduce_sim.cpp -x c oracle/tagmatch.c -lpthread -lrt -ldl
 
 .PHONY: all lib oracle oracle-core hostsim probe clean hostsim-asan hostsim-tsan

@@ -151,6 +151,19 @@ uint64_t sw_post_send(sw_ctx* ctx, sw_worker_t w, sw_ep_t ep, const void* ptr, s
 /* reference Client::recv / Server::recv (main.cpp:625-647, 1409-1431) */
 uint64_t sw_post_recv(sw_ctx* ctx, sw_worker_t w, void* ptr, size_t cap, uint64_t tag, uint64_t tag_mask,
                       int mem_kind);
+/* Element types of sw_post_recv_reduce */
+enum { SW_DTYPE_F32 = 1, SW_DTYPE_F16 = 2, SW_DTYPE_BF16 = 3, SW_DTYPE_F64 = 4, SW_DTYPE_I32 = 5, SW_DTYPE_I64 = 6 };
+/* A receive that ADDS the message into device memory instead of overwriting it (an extension: the reference
+ * has no such call).  Matches exactly like sw_post_recv.  The message's bytes, read as elements of `dtype`, are
+ * added element-wise into the first length / itemsize elements of `ptr`; completes as SW_OP_RECV with
+ * (sender_tag, length) once the sum is visible on every stream.  A message longer than `cap` fails with
+ * SW_STATUS_MESSAGE_TRUNCATED and one whose length is not a multiple of the element size with
+ * SW_STATUS_INVALID_PARAM; either way `ptr` is untouched and the sender's send succeeds.  Any number of reducing
+ * receives may target the same or overlapping memory at once (float sums in unspecified order).  Returns 0 with
+ * sw_last_error() set for an unknown dtype, a `cap` or `ptr` that is not a multiple of the element size, or a
+ * `ptr` that is not device memory of the context's device. */
+uint64_t sw_post_recv_reduce(sw_ctx* ctx, sw_worker_t w, void* ptr, size_t cap, uint64_t tag, uint64_t tag_mask,
+                             int dtype);
 /* reference flush / flush_ep (main.cpp:649-665, 1433-1471) */
 uint64_t sw_post_flush(sw_ctx* ctx, sw_worker_t w);
 uint64_t sw_post_flush_ep(sw_ctx* ctx, sw_worker_t w, sw_ep_t ep);

@@ -146,6 +146,7 @@ C_ABI = {
     "sw_close": (_u64, [_vp, _u64]),
     "sw_post_send": (_u64, [_vp, _u64, _u64, _vp, _sz, _u64, _int]),
     "sw_post_recv": (_u64, [_vp, _u64, _vp, _sz, _u64, _u64, _int]),
+    "sw_post_recv_reduce": (_u64, [_vp, _u64, _vp, _sz, _u64, _u64, _int]),
     "sw_post_flush": (_u64, [_vp, _u64]),
     "sw_post_flush_ep": (_u64, [_vp, _u64, _u64]),
     "sw_poll": (_int, [_vp, ctypes.POINTER(SwCompletion), _int]),
@@ -236,6 +237,47 @@ def as_buffer(obj: Any, writable: bool):
             raise TypeError("recv buffer is read-only")
         return int(ptr), int(shape[0]) * np.dtype(cai["typestr"]).itemsize, SW_MEM_DEVICE, obj
     raise TypeError(f"unsupported buffer type {type(obj)!r}: expected numpy.ndarray, torch.Tensor or a CUDA array")
+
+
+# element types of arecv_reduce (SW_DTYPE_* in include/starway_b200.h)
+SW_DTYPE_F32, SW_DTYPE_F16, SW_DTYPE_BF16, SW_DTYPE_F64, SW_DTYPE_I32, SW_DTYPE_I64 = 1, 2, 3, 4, 5, 6
+_REDUCE_TORCH = {"torch.float32": 1, "torch.float16": 2, "torch.bfloat16": 3, "torch.float64": 4, "torch.int32": 5,
+                 "torch.int64": 6}
+_REDUCE_TYPESTR = {"<f4": 1, "<f2": 2, "<f8": 4, "<i4": 5, "<i8": 6}  # bfloat16 has no typestr: torch only
+
+
+def as_reduce_buffer(obj: Any, device: int):
+    """-> (ptr, nbytes, dtype, keepalive) for arecv_reduce: a contiguous CUDA tensor on `device` (any shape) or a
+    contiguous ``__cuda_array_interface__`` object of a supported element type.  Anything else: TypeError."""
+    if _is_torch_tensor(obj):
+        dt = _REDUCE_TORCH.get(str(obj.dtype))
+        if dt is None:
+            raise TypeError(f"arecv_reduce: unsupported dtype {obj.dtype}")
+        if not obj.is_cuda or obj.device.index != device:
+            raise TypeError(f"arecv_reduce: the buffer must be a CUDA tensor on cuda:{device}")
+        if not obj.is_contiguous():
+            raise TypeError("arecv_reduce: the buffer must be contiguous")
+        return obj.data_ptr(), obj.numel() * obj.element_size(), dt, obj
+    cai = None if isinstance(obj, np.ndarray) else getattr(obj, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"arecv_reduce: expected a CUDA tensor or a CUDA array, got {type(obj)!r}")
+    dt = _REDUCE_TYPESTR.get(cai["typestr"])
+    if dt is None:
+        raise TypeError(f"arecv_reduce: unsupported typestr {cai['typestr']!r}")
+    shape = tuple(int(x) for x in cai["shape"])
+    itemsize = np.dtype(cai["typestr"]).itemsize
+    strides = cai.get("strides")
+    if strides is not None:
+        want, acc = [], itemsize
+        for dim in reversed(shape):
+            want.append(acc)
+            acc *= dim
+        if tuple(strides) != tuple(reversed(want)) and int(np.prod(shape)) > 1:
+            raise TypeError("arecv_reduce: the buffer must be contiguous")
+    ptr, readonly = cai["data"]
+    if readonly:
+        raise TypeError("arecv_reduce: the buffer is read-only")
+    return int(ptr), int(np.prod(shape)) * itemsize, dt, obj
 
 
 # ----------------------------------------------------------------------------- API factory
@@ -718,6 +760,29 @@ def bind(lib: ctypes.CDLL, default_device: Callable[[], int] | None = None, use_
                 op = _post_recv(ctx._h, self._w, ptr, n, tag & _U64MASK, tag_mask & _U64MASK, mem)
                 if not op:
                     raise RuntimeError(_err())
+                ctx._ops[op] = ("fut", loop, fut, keep, None)
+            if ctx._spin_loop is None:
+                ctx._kick()
+            return fut
+
+        def arecv_reduce(self, buffer, tag: int, tag_mask: int, loop: asyncio.AbstractEventLoop | None = None):
+            """Receive a message and ADD it into `buffer` instead of overwriting it (an extension beyond the
+            reference's API).  Matches exactly like `arecv`.  The message's bytes, read as elements of the buffer's
+            dtype, are added into the first ``length // itemsize`` elements; the future resolves to
+            ``(sender_tag, length)`` once the sum is visible on every stream.  `buffer`: a contiguous CUDA tensor on
+            the context's device (float32, float16, bfloat16, float64, int32, int64) or a contiguous
+            ``__cuda_array_interface__`` object; anything else raises TypeError.  Work queued on `buffer` must be
+            finished before the call."""
+            ctx = self._ctx
+            ptr, n, dtype, keep = as_reduce_buffer(buffer, ctx.device)
+            loop, fut = self._future(loop)
+            if not ctx._h:
+                raise RuntimeError("starway_b200 context is closed")
+            with ctx._lock:
+                op = lib.sw_post_recv_reduce(ctx._h, self._w, ptr, n, tag & _U64MASK, tag_mask & _U64MASK, dtype)
+                if not op:
+                    msg = _err()
+                    raise (TypeError if msg.startswith("recv_reduce:") else RuntimeError)(msg)
                 ctx._ops[op] = ("fut", loop, fut, keep, None)
             if ctx._spin_loop is None:
                 ctx._kick()

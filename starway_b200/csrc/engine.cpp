@@ -263,6 +263,33 @@ struct StagingPool {
   }
 };
 
+// Device landing blocks of reducing receives: the matcher copies an eager payload (at most SW_EAGER_MAX bytes) into
+// the receive's block, a reduce launch then adds it into the caller's buffer.  Fixed blocks carved from larger
+// allocations, so that thousands of receives in flight cost one slot each rather than a staging granule.
+struct LandingPool {
+  static constexpr size_t BLOCK = SW_SLOT_BYTES, PER_CHUNK = 256;
+  std::vector<void*> free_list, chunks;
+  void* get() {
+    if (free_list.empty()) {
+      uint8_t* chunk = (uint8_t*)swgpu::dev_alloc_raw(BLOCK * PER_CHUNK);
+      if (!chunk) return nullptr;
+      chunks.push_back(chunk);
+      for (size_t i = 0; i < PER_CHUNK; i++) free_list.push_back(chunk + i * BLOCK);
+    }
+    void* p = free_list.back();
+    free_list.pop_back();
+    return p;
+  }
+  void put(void* p) {
+    if (p) free_list.push_back(p);
+  }
+  void destroy() {
+    for (void* c : chunks) swgpu::dev_free(c);
+    chunks.clear();
+    free_list.clear();
+  }
+};
+
 // ============================================================================ pageable host buffers
 // cudaMemcpyAsync from / to pageable memory is a synchronous, single-threaded staging loop inside the driver
 // (slow, and it blocks the progress thread).  Large pageable buffers are moved by a few
@@ -443,6 +470,8 @@ struct RecvOp {
   void* pin_stage = nullptr;      // pageable host destination: page-locked landing zone of the device -> host copy
   size_t pin_stage_size = 0;
   std::atomic<int> pin_pending{0};
+  int dtype = 0;                  // reducing receive (sw_post_recv_reduce): SW_DT_* of the caller's buffer; 0: plain receive
+  void* landing = nullptr;        // reducing receive: device block the matcher copies an eager payload into
 };
 
 struct FlushOp {
@@ -467,6 +496,8 @@ struct BulkJob {
   Mapping* mapping = nullptr;
   bool failed = false;
   int32_t fail_status = 0;
+  int dtype = 0;            // reducing receive: dst += src with elements of this SW_DT_* type (0: copy)
+  bool src_ready = false;   // `src` is a local device address already (an eager payload in a landing block)
 };
 
 constexpr uint32_t EP_MAGIC = 0x53574550u, WORKER_MAGIC = 0x5357574Bu, DEAD_MAGIC = 0x44454144u;
@@ -668,6 +699,7 @@ struct BulkBlock {
   bool busy = false;
   std::vector<BulkJob> jobs;
   std::vector<SwSeg> tma, simt;  // scratch, capacity retained across launches
+  std::vector<SwSeg> rtma[7], rsimt[7];   // the same for reducing receives, indexed by SW_DT_*
   std::vector<void*> ce_dst;     // copies of this block made by the copy engine (device -> pinned host)
   std::vector<const void*> ce_src;
   std::vector<size_t> ce_len;
@@ -747,6 +779,7 @@ struct Ctx {
   std::deque<PostCopy> post_copies;
   HostPool host_pool;
   StagingPool staging;
+  LandingPool landing;
   PinnedPool pinned_pool;
   CopyPool copy_pool;
   std::atomic<int64_t> opt_copy_threads{4};   // helper threads for pageable host buffers (0: cudaMemcpyAsync on pageable memory)
@@ -922,6 +955,7 @@ void recv_release(Ctx* c, RecvOp* r) {
   if (r->pin_stage) c->pinned_pool.put(r->pin_stage, r->pin_stage_size);
   if (r->pinned_bounce) c->host_pool.put(r->pinned_bounce, r->cap);
   if (r->dev_staging) c->staging.put(r->dev_staging, r->staging_size);
+  c->landing.put(r->landing);
   delete r;
 }
 
@@ -1954,8 +1988,10 @@ void bulk_job_done(Ctx* c, BulkJob& j, int32_t status) {
   if (j.ep) {
     bool was_cancelled = j.ep->canceled_rts.erase(j.rts.send_seq) > 0;
     (void)was_cancelled;
-    // FIN: the sender's buffer is no longer needed (UCX: rendezvous ATS)
-    ctl_send(j.ep, CTL_FIN, status == SW_ERR_MESSAGE_TRUNCATED ? SW_OK : status, j.rts.send_seq);
+    // FIN: the sender's buffer is no longer needed (UCX: rendezvous ATS).  A message the receive refused (too long,
+    // or not a whole number of elements for a reducing receive) was still consumed: the send succeeded.
+    const bool refused = status == SW_ERR_MESSAGE_TRUNCATED || (j.dtype && status == SW_ERR_INVALID_PARAM);
+    ctl_send(j.ep, CTL_FIN, refused ? SW_OK : status, j.rts.send_seq);
   }
   release_mapping(c, j);
   if (j.w->bulk_inflight) j.w->bulk_inflight--;
@@ -1992,7 +2028,7 @@ bool pump_bulk(Ctx* c) {
       j.failed = true;
       j.fail_status = SW_ERR_CONNECTION_RESET;
     }
-    if (!j.failed) {
+    if (!j.failed && !j.src_ready) {
       if (j.rts.ctx_uuid == c->uuid && j.rts.src_pid == (uint32_t)getpid()) {
         j.src = j.rts.src_ptr;
       } else {
@@ -2048,6 +2084,10 @@ bool pump_bulk(Ctx* c) {
   b.ce_dst.clear();
   b.ce_src.clear();
   b.ce_len.clear();
+  for (int dt = 0; dt < 7; dt++) {
+    b.rtma[dt].clear();
+    b.rsimt[dt].clear();
+  }
   for (BulkJob& j : b.jobs) {
     uint64_t src = j.src, dst = j.dst, len = j.len;
     if (j.host_side && !j.src_host && c->opt_hostdst_ce.load()) {
@@ -2058,14 +2098,17 @@ bool pump_bulk(Ctx* c) {
       b.ce_len.push_back((size_t)len);
       continue;
     }
-    // receives into host memory were redirected to device staging at post time
+    // receives into host memory were redirected to device staging at post time (a reducing receive's destination
+    // is always device memory: host_side means a pinned-host source there)
     const bool tma_ok = !j.host_side || (!j.src_host && c->opt_hostdst_tma.load());   // device -> pinned host: bulk stores over PCIe
+    std::vector<SwSeg>& to_tma = j.dtype ? b.rtma[j.dtype] : tma;
+    std::vector<SwSeg>& to_simt = j.dtype ? b.rsimt[j.dtype] : simt;
     if (tune.mode == 0 && tma_ok && ((src | dst) & 15) == 0 && len >= 16) {
       uint64_t body = len & ~15ull;
-      for (uint64_t off = 0; off < body; off += seg) tma.push_back(SwSeg{src + off, dst + off, std::min(seg, body - off), 0});
-      if (len > body) simt.push_back(SwSeg{src + body, dst + body, len - body, 0});
+      for (uint64_t off = 0; off < body; off += seg) to_tma.push_back(SwSeg{src + off, dst + off, std::min(seg, body - off), 0});
+      if (len > body) to_simt.push_back(SwSeg{src + body, dst + body, len - body, 0});
     } else {
-      for (uint64_t off = 0; off < len; off += seg) simt.push_back(SwSeg{src + off, dst + off, std::min(seg, len - off), 0});
+      for (uint64_t off = 0; off < len; off += seg) to_simt.push_back(SwSeg{src + off, dst + off, std::min(seg, len - off), 0});
     }
   }
   uint32_t ntma = (uint32_t)tma.size(), nsimt = (uint32_t)simt.size();
@@ -2083,6 +2126,23 @@ bool pump_bulk(Ctx* c) {
     rc |= swgpu::launch_bulk(c->s_bulk, b.segs + ntma, nsimt, &t2);
   }
   if (!b.ce_dst.empty()) rc |= swgpu::memcpy_batch(b.ce_dst.data(), b.ce_src.data(), b.ce_len.data(), b.ce_dst.size(), c->s_bulk);
+  // reducing receives: one launch per element type and kernel, their segments after the copies' in b.segs
+  uint32_t nseg = ntma + nsimt, nred_tma = 0, nred_simt = 0;
+  for (int dt = 1; dt < 7; dt++) {
+    for (int simt_k = 0; simt_k < 2; simt_k++) {
+      const std::vector<SwSeg>& v = simt_k ? b.rsimt[dt] : b.rtma[dt];
+      if (v.empty()) continue;
+      memcpy(b.segs + nseg, v.data(), sizeof(SwSeg) * v.size());
+      swgpu::BulkTuning t2 = tune;
+      if (simt_k) {
+        t2.mode = 1;
+        t2.ctas_per_sm = 8;
+      }
+      rc |= swgpu::launch_reduce(c->s_bulk, b.segs + nseg, (uint32_t)v.size(), dt, &t2);
+      nseg += (uint32_t)v.size();
+      (simt_k ? nred_simt : nred_tma)++;
+    }
+  }
   if (rc) fprintf(stderr, "starway_b200: bulk launch failed: %s\n", swgpu::last_error());
   swgpu::event_record(b.timed ? b.ev : b.ev_fast, c->s_bulk);
   b.busy = true;
@@ -2090,6 +2150,8 @@ bool pump_bulk(Ctx* c) {
   std::lock_guard<std::mutex> lk(c->st_mu);
   if (ntma) c->stats.bulk_tma_launches++;
   if (nsimt) c->stats.bulk_simt_launches++;
+  c->stats.bulk_tma_launches += nred_tma;
+  c->stats.bulk_simt_launches += nred_simt;
   c->stats.bulk_jobs += b.jobs.size();
   c->stats.bulk_bytes += b.bytes;
   return true;
@@ -2174,6 +2236,32 @@ inline bool cq_ready(const SwCqEnt* e, uint64_t idx, int32_t* status) {
   return true;
 }
 
+// An eager message matched by a reducing receive sits in the receive's landing block: it becomes a bulk job from there
+// into the caller's buffer, launched with whatever else is pending (bulk_job_done then completes the receive).
+// Returns false when the receive completes as it is: not a reducing receive, an error, or length 0.
+bool reduce_landed(Ctx* c, Worker* w, uint64_t op_id, int32_t status, uint64_t tag, uint64_t len) {
+  auto it = w->recvs.find(op_id);
+  if (it == w->recvs.end() || !it->second->dtype || status != SW_OK || !len) return false;
+  RecvOp* r = it->second;
+  if (len % sw_dtype_size(r->dtype)) {
+    recv_finish(c, w, op_id, SW_ERR_INVALID_PARAM, tag, len);
+    return true;
+  }
+  BulkJob j;
+  j.w = w;
+  j.recv_op = op_id;
+  j.dst = (uint64_t)(uintptr_t)r->ptr;
+  j.cap = r->cap;
+  j.tag = tag;
+  j.len = len;
+  j.src = (uint64_t)(uintptr_t)r->landing;
+  j.src_ready = true;
+  j.dtype = r->dtype;
+  j.t_enq = now_s();
+  c->pending_bulk.push_back(j);
+  return true;
+}
+
 bool poll_progress_rings(Ctx* c, Worker* w) {
   bool any = false;
   // ---- eager completions
@@ -2183,7 +2271,7 @@ bool poll_progress_rings(Ctx* c, Worker* w) {
     int32_t status;
     if (!cq_ready(e, h, &status)) break;
     trace(c, "cqe_eager", e->op_id, e->len);
-    recv_finish(c, w, e->op_id, status, e->tag, e->len);
+    if (!reduce_landed(c, w, e->op_id, status, e->tag, e->len)) recv_finish(c, w, e->op_id, status, e->tag, e->len);
     h++;
   }
   if (h != w->cq_head) {
@@ -2228,10 +2316,17 @@ bool poll_progress_rings(Ctx* c, Worker* w) {
       auto rit = w->recvs.find(r.op_id);
       j.src_host = (r.rts.pad[0] & SW_RTS_PINNED_SRC) != 0;
       j.host_side = j.src_host || (rit != w->recvs.end() && rit->second->mem == MEM_PINNED);
+      if (rit != w->recvs.end() && rit->second->dtype) {
+        j.dtype = rit->second->dtype;
+        j.dst = (uint64_t)(uintptr_t)rit->second->ptr;   // reduced straight into the caller's buffer
+      }
     }
     if (r.status != SW_OK) {
       j.failed = true;
       j.fail_status = r.status;
+    } else if (j.dtype && r.len % sw_dtype_size(j.dtype)) {
+      j.failed = true;
+      j.fail_status = SW_ERR_INVALID_PARAM;
     }
     if (!j.ep || j.ep->retired || j.ep->ring_gen != gen) {
       // a request parked in the unexpected queue by a connection that has ended since: its source is gone
@@ -2287,6 +2382,18 @@ bool pump_progress(Ctx* c, Worker* w) {
            w->recvs.size() < SW_PQ_CAP / 2) {
       RecvOp* r = w->new_posts.front();
       uint64_t buf = (uint64_t)(uintptr_t)r->ptr;
+      if (r->dtype && r->cap) {
+        // reducing receive: an eager payload lands in a block of its own (reduce_landed), a rendezvous match takes the
+        // host path (pump_bulk reduces the sender's buffer straight into the caller's)
+        r->landing = c->landing.get();
+        buf = (uint64_t)(uintptr_t)r->landing;
+        if (!buf) {
+          w->new_posts.pop_front();
+          complete(c, w, r->op_id, SW_OP_RECV, SW_ERR_NO_MEMORY);
+          delete r;
+          continue;
+        }
+      }
       if (r->mem == SW_MEM_HOST && r->cap > HOST_BOUNCE_MAX) {
         swgpu::PtrInfo pi;
         swgpu::ptr_info(r->ptr, &pi);
@@ -2313,7 +2420,7 @@ bool pump_progress(Ctx* c, Worker* w) {
       p.buf = buf;
       p.cap = r->cap;
       p.op_id = r->op_id;
-      p.flags = r->mem == MEM_PINNED ? (uint32_t)SW_POST_HOSTPATH : 0u;
+      p.flags = r->mem == MEM_PINNED || r->dtype ? (uint32_t)SW_POST_HOSTPATH : 0u;
       if (r->pinned_bounce) p.flags |= SW_POST_HOSTBUF;
       p.pad = 0;
       if (!p.flags && r->cap > (uint64_t)c->opt_eager_max.load()) {
@@ -3314,6 +3421,7 @@ void sw_ctx_destroy(sw_ctx* ctx) {
   c->pinned_pool.destroy();
   c->host_pool.destroy();
   c->staging.destroy();
+  c->landing.destroy();
   swgpu::stream_destroy(c->s_put);
   swgpu::stream_destroy(c->s_bulk);
   if (c->efd >= 0) close(c->efd);
@@ -3618,6 +3726,47 @@ uint64_t sw_post_recv(sw_ctx* ctx, sw_worker_t wid, void* ptr, size_t cap, uint6
   r->tag = tag;
   r->mask = tag_mask;
   r->mem = cap ? classify_mem(ptr, mem_kind) : SW_MEM_DEVICE;
+  uint64_t id = r->op_id;
+  sq_push(c, SQ_RECV, w, r, &r->sqn);
+  return id;
+}
+
+static_assert((int)SW_DTYPE_F32 == (int)SW_DT_F32 && (int)SW_DTYPE_F16 == (int)SW_DT_F16 &&
+                  (int)SW_DTYPE_BF16 == (int)SW_DT_BF16 && (int)SW_DTYPE_F64 == (int)SW_DT_F64 &&
+                  (int)SW_DTYPE_I32 == (int)SW_DT_I32 && (int)SW_DTYPE_I64 == (int)SW_DT_I64,
+              "element type numbering of the C ABI and the kernels");
+
+uint64_t sw_post_recv_reduce(sw_ctx* ctx, sw_worker_t wid, void* ptr, size_t cap, uint64_t tag, uint64_t tag_mask,
+                             int dtype) {
+  Ctx* c = (Ctx*)ctx;
+  Worker* w = find_worker(c, wid);
+  if (!w || w->status.load(std::memory_order_acquire) != SW_ST_RUNNING) return not_running(w, "recv");
+  const uint32_t isz = sw_dtype_size(dtype);
+  if (!isz) {
+    set_error("recv_reduce: unknown element type");
+    return 0;
+  }
+  if (cap % isz || (uintptr_t)ptr % isz) {
+    set_error("recv_reduce: buffer address and size must be multiples of the element size");
+    return 0;
+  }
+  if (cap) {
+    swgpu::PtrInfo pi;
+    swgpu::ptr_info(ptr, &pi);
+    if (!pi.is_device || pi.device != c->device) {
+      set_error("recv_reduce: the buffer is not device memory of the context's device");
+      return 0;
+    }
+  }
+  RecvOp* r = new RecvOp();
+  r->op_id = c->next_id.fetch_add(1);
+  r->w = w;
+  r->ptr = (uint8_t*)ptr;
+  r->cap = cap;
+  r->tag = tag;
+  r->mask = tag_mask;
+  r->mem = SW_MEM_DEVICE;
+  r->dtype = dtype;
   uint64_t id = r->op_id;
   sq_push(c, SQ_RECV, w, r, &r->sqn);
   return id;

@@ -88,6 +88,11 @@ struct DoneFlag {
 };
 int launch_put(stream_t s, const SwPutDesc* descs, uint32_t n, const DoneFlag* done = nullptr);
 int launch_bulk(stream_t s, const SwSeg* segs, uint32_t nseg, const BulkTuning* tune);
+// dst[i] += src[i] over every segment, elements of type `dtype` (SW_DT_*); one launch serves one type.
+// tune->mode 0: TMA bulk reductions, every src / dst / len a multiple of 16 (sw_reduce_tma_kernel); 1: element-wise
+// atomics, dst and len multiples of the element size, src at any byte offset (sw_reduce_simt_kernel).
+// `segs` is read by the kernel (pinned host memory) and must stay valid until the launch completes.
+int launch_reduce(stream_t s, const SwSeg* segs, uint32_t nseg, int dtype, const BulkTuning* tune);
 
 // ---------------------------------------------------------------- resident progress path
 // 1: launch_progress / launch_pull start kernels that stay resident and watch device / host memory on their

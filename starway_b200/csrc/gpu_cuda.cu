@@ -78,6 +78,12 @@ int init(int device) {
   SW_CUDA(cudaFuncSetAttribute(sw_bulk_tma_jobs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
   SW_CUDA(cudaFuncSetAttribute(sw_bulk_tma_inline_kernel<SW_BULK_INLINE_SEGS_SMALL>,
                                cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
+  SW_CUDA(cudaFuncSetAttribute(sw_reduce_tma_kernel<SW_DT_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
+  SW_CUDA(cudaFuncSetAttribute(sw_reduce_tma_kernel<SW_DT_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
+  SW_CUDA(cudaFuncSetAttribute(sw_reduce_tma_kernel<SW_DT_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
+  SW_CUDA(cudaFuncSetAttribute(sw_reduce_tma_kernel<SW_DT_F64>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
+  SW_CUDA(cudaFuncSetAttribute(sw_reduce_tma_kernel<SW_DT_I32>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
+  SW_CUDA(cudaFuncSetAttribute(sw_reduce_tma_kernel<SW_DT_I64>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem_optin));
   return 0;
 }
 int bind_thread(int device) {
@@ -463,6 +469,49 @@ int launch_bulk(stream_t s, const SwSeg* segs, uint32_t nseg, const BulkTuning* 
     uint32_t grid = (uint32_t)(g_sms * (t->ctas_per_sm > 0 ? t->ctas_per_sm : 4));
     if (grid > nseg) grid = nseg;
     sw_bulk_simt_kernel<<<grid, 256, 0, (cudaStream_t)s>>>(segs, nseg);
+  }
+  SW_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int DT>
+static void launch_reduce_as(cudaStream_t s, const SwSeg* segs, uint32_t nseg, int tma, uint32_t grid, size_t smem,
+                             uint32_t sb, uint32_t stages) {
+  if (tma)
+    sw_reduce_tma_kernel<DT><<<grid, 32, smem, s>>>(segs, nseg, sb, stages);
+  else
+    sw_reduce_simt_kernel<DT><<<grid, 256, 0, s>>>(segs, nseg);
+}
+
+int launch_reduce(stream_t s, const SwSeg* segs, uint32_t nseg, int dtype, const BulkTuning* t) {
+  if (!nseg) return 0;
+  const int tma = t->mode == 0;
+  int stages = t->stages < 2 ? 2 : (t->stages > SW_BULK_MAX_STAGES ? SW_BULK_MAX_STAGES : t->stages);
+  int sb = t->stage_bytes & ~15;
+  if (sb < 1024) sb = 1024;
+  const size_t smem = (size_t)stages * sb;
+  int ctas = t->ctas_per_sm > 0 ? t->ctas_per_sm : 1;
+  if (tma) {
+    if ((int)smem > g_max_smem_optin) {
+      g_err = "bulk tuning exceeds shared memory";
+      return -1;
+    }
+    const int fit = (int)((size_t)g_smem_per_sm / (smem + 1024 + 128));   // CTAs of this size resident per SM
+    if (ctas > fit) ctas = fit < 1 ? 1 : fit;
+  }
+  uint32_t grid = (uint32_t)(g_sms * ctas);
+  if (grid > nseg) grid = nseg;
+  cudaStream_t cs = (cudaStream_t)s;
+  switch (dtype) {
+    case SW_DT_F32: launch_reduce_as<SW_DT_F32>(cs, segs, nseg, tma, grid, smem, (uint32_t)sb, (uint32_t)stages); break;
+    case SW_DT_F16: launch_reduce_as<SW_DT_F16>(cs, segs, nseg, tma, grid, smem, (uint32_t)sb, (uint32_t)stages); break;
+    case SW_DT_BF16: launch_reduce_as<SW_DT_BF16>(cs, segs, nseg, tma, grid, smem, (uint32_t)sb, (uint32_t)stages); break;
+    case SW_DT_F64: launch_reduce_as<SW_DT_F64>(cs, segs, nseg, tma, grid, smem, (uint32_t)sb, (uint32_t)stages); break;
+    case SW_DT_I32: launch_reduce_as<SW_DT_I32>(cs, segs, nseg, tma, grid, smem, (uint32_t)sb, (uint32_t)stages); break;
+    case SW_DT_I64: launch_reduce_as<SW_DT_I64>(cs, segs, nseg, tma, grid, smem, (uint32_t)sb, (uint32_t)stages); break;
+    default:
+      g_err = "launch_reduce: unknown element type";
+      return -1;
   }
   SW_CUDA(cudaGetLastError());
   return 0;

@@ -6,9 +6,14 @@
 //   sw_bulk_tma_kernel  rendezvous / loopback bulk copy, cp.async.bulk global->smem->global
 //                       with an mbarrier pipeline (replaces the rendezvous leg of ucp_tag_send_nbx)
 //   sw_bulk_simt_kernel generic-alignment bulk copy (fallback + comparison)
+//   sw_reduce_tma_kernel  reducing receive (arecv_reduce): the bulk-copy pipeline with its smem->global store
+//                       replaced by cp.reduce.async.bulk .add, so dst += src costs a copy plus one read of dst
+//   sw_reduce_simt_kernel the same sum element by element with atomics: tails, generic alignment, host sources
 //
-// Pure data movement and uint64 xor/and/compare: no tensor cores, no floating point.
+// Data movement and uint64 xor/and/compare; the only arithmetic is the element-wise add of the reduce kernels.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "sw_device.h"
@@ -225,9 +230,16 @@ __global__ void __launch_bounds__(SW_PUT_INLINE * 32) sw_put_inline_kernel(const
 // multiples of 16 B (the host routes anything else to sw_bulk_simt_kernel).
 constexpr int SW_BULK_MAX_STAGES = 8;
 
+// The smem -> global step of the pipeline: a plain bulk store (copies) or a bulk reduction (SwBulkReduceStore).
+struct SwBulkCopyStore {
+  static __device__ __forceinline__ void store(void* gdst, const void* smem_src, uint32_t bytes) {
+    sw_bulk_s2g(gdst, smem_src, bytes);
+  }
+};
+
 // The copy pipeline, shared by the entry points below.  `next(src, dst, bytes)` yields this CTA's
 // pieces (each at most stage_bytes, 16-byte aligned) until it returns false.
-template <class Next>
+template <class Store = SwBulkCopyStore, class Next>
 __device__ __forceinline__ void sw_bulk_tma_pipeline(Next next, uint32_t stage_bytes, uint32_t nstages) {
   extern __shared__ __align__(128) uint8_t sw_smem[];
   __shared__ __align__(8) uint64_t full[SW_BULK_MAX_STAGES];
@@ -267,7 +279,7 @@ __device__ __forceinline__ void sw_bulk_tma_pipeline(Next next, uint32_t stage_b
     if (done == issued) break;
     const uint32_t stg = done % nstages;
     sw_mbar_wait(&full[stg], (done / nstages) & 1);
-    sw_bulk_s2g(reinterpret_cast<void*>(st_dst[stg]), sw_smem + size_t(stg) * stage_bytes, st_bytes[stg]);
+    Store::store(reinterpret_cast<void*>(st_dst[stg]), sw_smem + size_t(stg) * stage_bytes, st_bytes[stg]);
     sw_bulk_commit();
     done++;
   }
@@ -275,14 +287,14 @@ __device__ __forceinline__ void sw_bulk_tma_pipeline(Next next, uint32_t stage_b
 }
 
 // Segment-list source: CTA b walks segments b, b + gridDim.x, ...
-template <class SegAt>
+template <class Store = SwBulkCopyStore, class SegAt>
 __device__ __forceinline__ void sw_bulk_tma_body(SegAt seg_at, uint32_t nseg, uint32_t stage_bytes, uint32_t nstages) {
   uint32_t s = blockIdx.x;
   uint64_t off = 0;
   SwSeg cur;
   cur.src = cur.dst = cur.len = 0;
   if (threadIdx.x == 0 && s < nseg) cur = seg_at(s);
-  sw_bulk_tma_pipeline(
+  sw_bulk_tma_pipeline<Store>(
       [&](uint64_t& src, uint64_t& dst, uint32_t& bytes) -> bool {
         while (s < nseg && off >= cur.len) {
           s += gridDim.x;
@@ -341,5 +353,92 @@ __global__ void __launch_bounds__(256) sw_bulk_simt_kernel(const SwSeg* __restri
     const SwSeg g = segs[s];
     sw_copy(reinterpret_cast<uint8_t*>(g.dst), reinterpret_cast<const uint8_t*>(g.src), g.len, threadIdx.x,
             blockDim.x);
+  }
+}
+
+// ------------------------------------------------------------------ reducing receive: dst += src
+// Element type and atomic add of each SW_DT_* type.  f32 uses a compare-and-swap loop around a plain add: the
+// scalar red.global.add.f32 flushes subnormals (SASS REDG.E.ADD.F32.FTZ.RN) while the bulk reduction does not,
+// and both paths must produce the same bits.  The f16 / bf16 atomics are .noftz, f64 / s32 / u64 have no flush.
+template <int DT> struct SwRedType;
+template <> struct SwRedType<SW_DT_F32> { typedef float T; };
+template <> struct SwRedType<SW_DT_F16> { typedef __half T; };
+template <> struct SwRedType<SW_DT_BF16> { typedef __nv_bfloat16 T; };
+template <> struct SwRedType<SW_DT_F64> { typedef double T; };
+template <> struct SwRedType<SW_DT_I32> { typedef int T; };
+template <> struct SwRedType<SW_DT_I64> { typedef unsigned long long T; };   // two's complement: u64 add == s64 add
+
+__device__ __forceinline__ void sw_red_add(float* p, float v) {
+  unsigned int* a = reinterpret_cast<unsigned int*>(p);
+  unsigned int old = *reinterpret_cast<volatile unsigned int*>(a), seen;
+  do {
+    seen = old;
+    old = atomicCAS(a, seen, __float_as_uint(__fadd_rn(__uint_as_float(seen), v)));
+  } while (old != seen);
+}
+__device__ __forceinline__ void sw_red_add(__half* p, __half v) { atomicAdd(p, v); }
+__device__ __forceinline__ void sw_red_add(__nv_bfloat16* p, __nv_bfloat16 v) { atomicAdd(p, v); }
+__device__ __forceinline__ void sw_red_add(double* p, double v) {
+  asm volatile("red.global.add.f64 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "d"(v) : "memory");
+}
+__device__ __forceinline__ void sw_red_add(int* p, int v) {
+  asm volatile("red.global.add.s32 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sw_red_add(unsigned long long* p, unsigned long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "l"(v) : "memory");
+}
+
+// Bulk reduction shared -> global (SASS: UBLKRED.G.S.ADD.<type>), tracked by bulk async-groups like sw_bulk_s2g.
+template <int DT> struct SwBulkReduceStore;
+#define SW_BULK_REDUCE_STORE(DT, OP)                                                                         \
+  template <> struct SwBulkReduceStore<DT> {                                                                 \
+    static __device__ __forceinline__ void store(void* gdst, const void* smem_src, uint32_t bytes) {         \
+      asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add." OP " [%0], [%1], %2;" ::"l"(    \
+                       __cvta_generic_to_global(gdst)),                                                      \
+                   "r"(sw_smem_u32(smem_src)), "r"(bytes)                                                    \
+                   : "memory");                                                                              \
+    }                                                                                                        \
+  };
+SW_BULK_REDUCE_STORE(SW_DT_F32, "f32")
+SW_BULK_REDUCE_STORE(SW_DT_F16, "noftz.f16")
+SW_BULK_REDUCE_STORE(SW_DT_BF16, "noftz.bf16")
+SW_BULK_REDUCE_STORE(SW_DT_F64, "f64")
+SW_BULK_REDUCE_STORE(SW_DT_I32, "s32")
+SW_BULK_REDUCE_STORE(SW_DT_I64, "u64")
+#undef SW_BULK_REDUCE_STORE
+
+// Segment list in pinned host memory, every src / dst / len a multiple of 16 (the host routes the rest to
+// sw_reduce_simt_kernel).  Each element's add is performed by the memory system as its own atomic operation, so
+// segments of one launch may overlap in dst.
+template <int DT>
+__global__ void __launch_bounds__(32) sw_reduce_tma_kernel(const SwSeg* __restrict__ segs, uint32_t nseg,
+                                                           uint32_t stage_bytes, uint32_t nstages) {
+  sw_bulk_tma_body<SwBulkReduceStore<DT>>([segs](uint32_t i) { return segs[i]; }, nseg, stage_bytes, nstages);
+}
+
+// One CTA per segment (grid-stride), one element per thread and step.  dst and len are multiples of the element
+// size; src may sit at any byte offset (a sender's buffer is any slice of a byte tensor).
+template <int DT>
+__global__ void __launch_bounds__(256) sw_reduce_simt_kernel(const SwSeg* __restrict__ segs, uint32_t nseg) {
+  typedef typename SwRedType<DT>::T T;
+  constexpr uint32_t S = sizeof(T);
+  for (uint32_t s = blockIdx.x; s < nseg; s += gridDim.x) {
+    const SwSeg g = segs[s];
+    T* dst = reinterpret_cast<T*>(g.dst);
+    const uint64_t n = g.len / S;
+    if ((g.src & (S - 1)) == 0) {
+      const T* src = reinterpret_cast<const T*>(g.src);
+      for (uint64_t i = threadIdx.x; i < n; i += blockDim.x) sw_red_add(dst + i, src[i]);
+    } else {
+      const uint8_t* src = reinterpret_cast<const uint8_t*>(g.src);
+      for (uint64_t i = threadIdx.x; i < n; i += blockDim.x) {
+        uint8_t b[S];
+#pragma unroll
+        for (uint32_t k = 0; k < S; k++) b[k] = src[i * S + k];
+        T v;
+        memcpy(&v, b, S);
+        sw_red_add(dst + i, v);
+      }
+    }
   }
 }

@@ -89,6 +89,17 @@ enum : int32_t {
   SW_ERR_BUSY = -15,
 };
 
+// Element types of a reducing receive (same numbering as SW_DTYPE_* in include/starway_b200.h).
+enum : int { SW_DT_F32 = 1, SW_DT_F16 = 2, SW_DT_BF16 = 3, SW_DT_F64 = 4, SW_DT_I32 = 5, SW_DT_I64 = 6 };
+SW_HD inline uint32_t sw_dtype_size(int dt) {   // 0: unknown type
+  switch (dt) {
+    case SW_DT_F32: case SW_DT_I32: return 4;
+    case SW_DT_F16: case SW_DT_BF16: return 2;
+    case SW_DT_F64: case SW_DT_I64: return 8;
+    default: return 0;
+  }
+}
+
 struct SwRndvRec {  // a rendezvous match handed to the host (inside SwHrEnt): the receiver pulls the payload
   uint64_t op_id;
   uint64_t dst;
