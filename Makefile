@@ -16,6 +16,7 @@ FASTPATH  := starway_b200/_fastpath.so
 PYINC     := $(shell python -c "import sysconfig; print(sysconfig.get_paths()['include'])")
 PROBE     := tests/gpu_probe/sw_probe
 ABIBENCH  := tests/gpu_probe/abi_bench
+KTEST     := tests/gpu_kernels/libsw_kernels_test.so
 
 ENGINE_SRCS := $(CSRC)/engine.cpp
 ENGINE_HDRS := $(CSRC)/gpu.h $(CSRC)/sw_device.h include/starway_b200.h
@@ -26,7 +27,7 @@ lib: $(LIB) $(FASTPATH)
 oracle: $(ORACLE) $(CPUENG)
 oracle-core: $(ORACLE)
 hostsim: $(HOSTSIM)
-probe: $(PROBE) $(ABIBENCH)
+probe: $(PROBE) $(ABIBENCH) $(KTEST)
 
 build/gpu_cuda.o: $(CSRC)/gpu_cuda.cu $(CSRC)/kernels.cuh $(CSRC)/progress.cuh $(CSRC)/gpu.h $(CSRC)/sw_device.h $(CSRC)/bulk_jobs.h
 	@mkdir -p build
@@ -76,11 +77,16 @@ $(HOSTSIM): build/engine_sim.o build/gpu_sim.o build/reduce_sim.o build/tagmatch
 $(PROBE): tests/gpu_probe/probe.cu build/gpu_cuda.o
 	$(NVCC) $(NVFLAGS) -o $@ tests/gpu_probe/probe.cu build/gpu_cuda.o
 
+# Flat C entry points over the CUDA backend for tests/test_gpu_kernels.py (one kernel per launch, shapes chosen by
+# the test); test-only, never linked into $(LIB)
+$(KTEST): tests/gpu_kernels/kernels_test.cu tests/gpu_kernels/exports.map build/gpu_cuda.o $(CSRC)/gpu.h $(CSRC)/sw_device.h
+	$(NVCC) $(NVFLAGS) -shared -Xlinker -Bsymbolic -Xlinker --version-script=tests/gpu_kernels/exports.map -o $@ tests/gpu_kernels/kernels_test.cu build/gpu_cuda.o -lpthread -lrt
+
 $(ABIBENCH): tests/gpu_probe/abi_bench.cpp $(LIB) include/starway_b200.h
 	$(CXX) -O2 -std=c++17 -I/usr/local/cuda/include -o $@ tests/gpu_probe/abi_bench.cpp -Lstarway_b200 -lstarway_b200 -L/usr/local/cuda/lib64 -lcudart -Wl,-rpath,'$$ORIGIN/../../starway_b200' -Wl,-rpath,/usr/local/cuda/lib64
 
 clean:
-	rm -rf build $(LIB) $(FASTPATH) $(ORACLE) $(CPUENG) $(HOSTSIM) $(PROBE) $(ABIBENCH)
+	rm -rf build $(LIB) $(FASTPATH) $(ORACLE) $(CPUENG) $(HOSTSIM) $(PROBE) $(ABIBENCH) $(KTEST)
 
 # Instrumented builds of the host-logic simulator (same sources) for sanitizer runs of the CPU suite:
 #   make hostsim-asan && SW_HOSTSIM_LIB=$PWD/build/asan/libstarway_hostsim.so ASAN_OPTIONS=detect_leaks=0 \

@@ -70,6 +70,10 @@ namespace {
 thread_local std::string g_last_error;
 void set_error(const std::string& s) { g_last_error = s; }
 
+// A pull grid of one CTA is CTA 0 alone, which completes batches but copies nothing: the control kernel would still
+// hand rendezvous matches to it (pull_ctas != 0) and those receives would never complete.
+const char* const kPullCtasOne = "1 is not a valid value: the pull kernel needs CTA 0 plus at least one copy CTA";
+
 double now_s() {
   return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
@@ -3307,7 +3311,12 @@ sw_ctx* sw_ctx_create(int device) {
   if (const char* e = getenv("STARWAY_LINGER_US")) c->opt_linger_us = std::max<int64_t>(1, atoll(e));
   if (const char* e = getenv("STARWAY_MAX_LIFE_US")) c->opt_max_life_us = std::max<int64_t>(10, atoll(e));
   if (const char* e = getenv("STARWAY_ARMED_MS")) c->opt_armed_ms = std::max<int64_t>(0, atoll(e));
-  if (const char* e = getenv("STARWAY_PULL_CTAS")) c->opt_pull_ctas = std::max<int64_t>(0, atoll(e));
+  if (const char* e = getenv("STARWAY_PULL_CTAS")) {
+    if (atoll(e) == 1)
+      fprintf(stderr, "starway_b200: STARWAY_PULL_CTAS=1 ignored: %s\n", kPullCtasOne);
+    else
+      c->opt_pull_ctas = std::max<int64_t>(0, atoll(e));
+  }
   // environment knobs
   if (const char* e = getenv("STARWAY_EAGER_MAX")) c->opt_eager_max = std::min<int64_t>(atoll(e), SW_EAGER_MAX);
   if (const char* e = getenv("STARWAY_RING_SLOTS")) c->opt_ring_slots = std::max<int64_t>(atoll(e), 4);
@@ -3328,7 +3337,7 @@ sw_ctx* sw_ctx_create(int device) {
       const std::string kv = all.substr(pos, end - pos);
       const size_t eq = kv.find('=');
       if (eq != std::string::npos && sw_set_option((sw_ctx*)c, kv.substr(0, eq).c_str(), atoll(kv.c_str() + eq + 1)) != 0)
-        fprintf(stderr, "starway_b200: STARWAY_OPTS: unknown option '%s'\n", kv.substr(0, eq).c_str());
+        fprintf(stderr, "starway_b200: STARWAY_OPTS: '%s' ignored: unknown option or invalid value\n", kv.c_str());
       pos = end + 1;
     }
   }
@@ -3467,11 +3476,11 @@ int sw_set_option(sw_ctx* ctx, const char* key, int64_t value) {
   else if (k == "linger_us") c->opt_linger_us = std::max<int64_t>(1, value);
   else if (k == "max_life_us") c->opt_max_life_us = std::max<int64_t>(10, value);
   else if (k == "armed_ms") c->opt_armed_ms = std::max<int64_t>(0, value);
-  else if (k == "pull_ctas") c->opt_pull_ctas = std::max<int64_t>(0, value);
+  else if (k == "pull_ctas" && value != 1) c->opt_pull_ctas = std::max<int64_t>(0, value);
   else if (k == "resident_puts") c->opt_resident_puts = std::max<int64_t>(0, value);
   else if (k == "yield_us") c->opt_yield_us = std::max<int64_t>(0, value);
   else {
-    set_error("unknown option " + k);
+    set_error(k == "pull_ctas" ? "pull_ctas: " + std::string(kPullCtasOne) : "unknown option " + k);
     return -1;
   }
   return 0;

@@ -88,6 +88,9 @@ struct DoneFlag {
 };
 int launch_put(stream_t s, const SwPutDesc* descs, uint32_t n, const DoneFlag* done = nullptr);
 int launch_bulk(stream_t s, const SwSeg* segs, uint32_t nseg, const BulkTuning* tune);
+// largest stages * stage_bytes a TMA bulk copy or reduction accepts (the device's opt-in shared memory per block less
+// the kernels' static shared memory); launch_bulk / launch_reduce return -1 above it.  0 before init().
+int bulk_smem_limit();
 // dst[i] += src[i] over every segment, elements of type `dtype` (SW_DT_*); one launch serves one type.
 // tune->mode 0: TMA bulk reductions, every src / dst / len a multiple of 16 (sw_reduce_tma_kernel); 1: element-wise
 // atomics, dst and len multiples of the element size, src at any byte offset (sw_reduce_simt_kernel).

@@ -92,6 +92,7 @@ int bind_thread(int device) {
 }
 int sm_count() { return g_sms; }
 int clock_mhz() { return g_clk_mhz; }
+int bulk_smem_limit() { return g_max_smem_optin; }
 int device_pci_bus_id(int device, char* out, int cap) {
   if (cap < 16) return -1;
   cudaError_t r = cudaDeviceGetPCIBusId(out, cap, device);

@@ -338,6 +338,46 @@ def test_options_from_the_environment(port):
     assert "no_such_option" in out.stderr
 
 
+def test_pull_ctas_of_one_is_refused(sim_api):
+    """A pull grid of one CTA is CTA 0 alone, which copies nothing: rendezvous receives handed to it would never
+    complete.  `sw_set_option("pull_ctas", 1)` fails and leaves the value as it was; 0 and 2 are accepted.
+    STARWAY_PULL_CTAS=1 is ignored with a warning."""
+    import os
+    import subprocess
+    import sys
+
+    ctx = sim_api.get_context()
+    old = ctx.get_option("pull_ctas")
+    try:
+        ctx.set_option("pull_ctas", 2)
+        with pytest.raises(ValueError, match="pull_ctas"):
+            ctx.set_option("pull_ctas", 1)
+        assert ctx.get_option("pull_ctas") == 2
+        ctx.set_option("pull_ctas", 0)
+        assert ctx.get_option("pull_ctas") == 0
+    finally:
+        ctx.set_option("pull_ctas", old)
+
+    code = ("from tests import hostsim; sw = hostsim.load(); c = sw.get_context(); "
+            "print(c.get_option('pull_ctas')); sw.shutdown()")
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    outs = {}
+    for name, value in (("STARWAY_PULL_CTAS", "1"), ("STARWAY_OPTS", "pull_ctas=1"), ("STARWAY_PULL_CTAS", "3")):
+        env = dict(os.environ, STARWAY_QUIET="1")
+        env.pop("STARWAY_PULL_CTAS", None)
+        env.pop("STARWAY_OPTS", None)
+        env[name] = value
+        out = subprocess.run([sys.executable, "-c", code], env=env, cwd=root, capture_output=True, text=True, timeout=120)
+        assert out.returncode == 0, out.stderr
+        outs[(name, value)] = (int(out.stdout.split()[-1]), out.stderr)
+    default = outs[("STARWAY_PULL_CTAS", "1")][0]
+    assert default not in (0, 1), outs
+    assert outs[("STARWAY_OPTS", "pull_ctas=1")][0] == default, outs
+    assert outs[("STARWAY_PULL_CTAS", "3")][0] == 3 and "ignored" not in outs[("STARWAY_PULL_CTAS", "3")][1], outs
+    for key in (("STARWAY_PULL_CTAS", "1"), ("STARWAY_OPTS", "pull_ctas=1")):
+        assert "pull_ctas" in outs[key][1].lower() and "ignored" in outs[key][1], outs
+
+
 @pytest.mark.parametrize("bound", [1, 2])
 def test_mapping_cache_eviction(sim_api, port, bound):
     """More peer allocations than the receiver keeps mapped (`max_mappings`): the least recently used idle mappings are
